@@ -93,10 +93,31 @@ typedef struct tsnap_copy_desc {
     int32_t dst_dtype;  /* enum tsnap_dtype; != src_dtype fuses a cast (north star "cast in the pack kernel") */
     int32_t src_space;  /* enum tsnap_space */
     int32_t dst_space;  /* enum tsnap_space */
-    int32_t reserved;
+    int32_t reserved;   /* quantisation scheme, TSNAP_QSCHEME_*; 0 for every other copy */
     double q_scale;        /* dst_dtype TSNAP_QINT8 / TSNAP_QUINT8 only */
-    int64_t q_zero_point;
+    int64_t q_zero_point;  /* TSNAP_QSCHEME_PER_CHANNEL: address of a host tsnap_qchannel, read during the call */
 } tsnap_copy_desc;
+
+/* Quantisation schemes (tsnap_copy_desc.reserved).
+ *   PER_TENSOR (0): q_scale / q_zero_point as above.
+ *   PER_CHANNEL (1): the reference's per-channel format (T:serialization.py:366-477)
+ *       [axis: int64][int_repr bytes, C order][scales: float64 x C][zero_points: int64 x C]
+ *     save   : src = float view (DEVICE or HOST), dst_dtype QINT8 / QUINT8, dst WIRE at body_addr.  The engine computes
+ *              each channel's (scale, zero_point) from the source — qint8: amax / 127 (1.0 when 0), zero point 0;
+ *              quint8: (max(hi, 0) - min(lo, 0)) / 255 (1.0 when 0), zero point round_half_even(-min(lo, 0) / scale) —
+ *              and writes the axis header, the int body and both parameter arrays.  A NaN or Inf fails the call / job.
+ *     restore: src_dtype QINT8 / QUINT8 in WIRE (the piece or a sub-box of it), dst = float view of any float dtype:
+ *              float((q - zero_point) * scale) converted to the destination dtype.
+ *   The channel of wire element e is ((e - body_addr) / inner) % channels. */
+#define TSNAP_QSCHEME_PER_TENSOR 0
+#define TSNAP_QSCHEME_PER_CHANNEL 1
+typedef struct tsnap_qchannel {
+    int64_t channels;     /* C = piece shape[axis]                                            */
+    int64_t inner;        /* prod(piece shape after axis)                                     */
+    uint64_t body_addr;   /* WIRE offset of the piece's first int element (the header is 8 B before it) */
+    uint64_t params_addr; /* WIRE offset of scales[C]; zero_points[C] follow                  */
+    int64_t axis;         /* written into the header on save                                  */
+} tsnap_qchannel;
 
 typedef struct tsnap_engine tsnap_engine;
 typedef struct tsnap_job tsnap_job;

@@ -1,8 +1,10 @@
 """Isolated launches of every kernel mode through the C-ABI stager seam, for ncu captures and CUDA-event roofline
 numbers:  dense (bulk/TMA), column shard (rows/TMA), odd-alignment slab member (LSU contig), transpose (LSU tiled),
-fp32->bf16 cast (LSU cast), short strided runs (LSU strided).  Prints one JSON line per case with the kernel's
+fp32->bf16 cast (LSU cast), short strided runs (LSU strided), per-channel int8 quantisation (statistics + parameters +
+quantising pack) along dim 0 and dim 1, and its dequantising scatter.  Prints one JSON line per case with the kernel's
 CUDA-event time and achieved GB/s against the measured HBM copy peak (MEASURED_PEAKS.json; else the H100 SXM data
-sheet's 3.35 TB/s).
+sheet's 3.35 TB/s).  A per-channel save reads its source twice (statistics, then the pack): its algorithmic bytes are
+both reads, the 1-byte elements written and the 16 bytes of parameters per channel.
 
     python tools/kernel_cases.py [--case NAME] [--reps N]
     ncu --set full --clock-control none --import-source on -k regex:tsnap -o kernels python tools/kernel_cases.py --reps 1
@@ -37,11 +39,17 @@ def cases():
     yield "cast_fp32_to_bf16_1GiB", [(base, 0, torch.bfloat16)], GiB // 2, GiB + GiB // 2
     short = base.view(1 << 22, 64)[:, 8:40]  # 128 B runs: below the copy-engine threshold
     yield "strided_128B_runs", [(short, 0, None)], short.numel() * 4, 2 * short.numel() * 4
+    m = base.view(262144, 1024)
+    for axis in (0, 1):
+        C = m.shape[axis]
+        yield f"qchannel_fp32_axis{axis}_1GiB", [(m, 8, torch.qint8, axis)], 8 + m.numel() + 16 * C, 2 * GiB + m.numel() + 16 * C
+    hb = torch.empty(524288, 1024, dtype=torch.bfloat16, device=dev).normal_()  # finite values (reinterpreted fp32 bits are not)
+    yield "qchannel_bf16_axis0_1GiB", [(hb, 8, torch.qint8, 0)], 8 + hb.numel() + 16 * 524288, 2 * GiB + hb.numel() + 16 * 524288
 
 for name, members, nbytes, algo in cases():
     if args.case not in ("all", name):
         continue
-    descs = [N.save_desc(t, off, wire_dtype=wd) for t, off, wd in members]
+    descs = [N.save_desc(m[0], m[1], wire_dtype=m[2], axis=m[3] if len(m) > 3 else None) for m in members]
     total = nbytes + 16
     best = None
     for rep in range(args.reps + 1):
@@ -53,4 +61,22 @@ for name, members, nbytes, algo in cases():
     print(json.dumps({"case": name, "kernel_ms": round(st["kernel_ms"], 4), "bulk_ms": round(st["kernel_bulk_ms"], 4), "rows_ms": round(st["kernel_rows_ms"], 4),
                       "lsu_ms": round(st["kernel_lsu_ms"], 4), "tiles": [st["n_tiles_bulk"], st["n_tiles_rows"], st["n_tiles_lsu"]],
                       "algorithmic_bytes": algo, "gbs": round(algo / 1e6 / st["kernel_ms"], 1), "frac_of_measured_peak": round(algo / 1e6 / st["kernel_ms"] / peak, 3)}), flush=True)
+
+# dequantising scatter: the 1 GiB fp32 [262144, 1024] target of an axis-0 int8 image already in device memory
+if args.case in ("all", "qchannel_dequant_fp32_axis0_1GiB"):
+    dst = torch.empty(262144, 1024, dtype=torch.float32, device=dev)
+    wire = torch.empty(8 + dst.numel() + 16 * 262144, dtype=torch.uint8, device=dev)
+    sb = eng.stage([N.save_desc(dst.uniform_(), 8, wire_dtype=torch.qint8, axis=0)], wire.numel(), keepalive=[dst])
+    wire.copy_(torch.frombuffer(bytearray(sb.wait()), dtype=torch.uint8).to(dev)); sb.release()
+    desc = N.per_channel(N.load_desc(dst, 8, wire_dtype=torch.qint8), [262144, 1024], 0, 8)
+    ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
+    times = []
+    for rep in range(args.reps + 1):
+        ev[0].record(); eng.scatter_device(wire, [desc]); ev[1].record(); torch.cuda.synchronize()
+        if rep:
+            times.append(ev[0].elapsed_time(ev[1]))
+    ms = min(times)
+    algo = dst.numel() + 16 * 262144 + dst.numel() * 4
+    print(json.dumps({"case": "qchannel_dequant_fp32_axis0_1GiB", "kernel_ms": round(ms, 4), "note": "CUDA events around tsnap_scatter_device (table upload + launch + kernel)",
+                      "algorithmic_bytes": algo, "gbs": round(algo / 1e6 / ms, 1), "frac_of_measured_peak": round(algo / 1e6 / ms / peak, 3)}), flush=True)
 eng.close()

@@ -70,6 +70,52 @@ class CopyDesc(C.Structure):
     ]
 
 
+# tsnap_copy_desc.reserved: quantisation scheme
+QSCHEME_PER_TENSOR, QSCHEME_PER_CHANNEL = 0, 1
+
+
+class QChannel(C.Structure):
+    """tsnap_qchannel: where the per-channel format's parts of one piece sit in the wire image."""
+
+    _fields_ = [
+        ("channels", C.c_int64),
+        ("inner", C.c_int64),
+        ("body_addr", C.c_uint64),
+        ("params_addr", C.c_uint64),
+        ("axis", C.c_int64),
+    ]
+
+
+def per_channel(d: CopyDesc, shape: Sequence[int], axis: int, body: int) -> CopyDesc:
+    """Marks ``d`` as a per-channel copy of the piece of ``shape`` whose int body starts at wire offset ``body`` (the
+    axis header sits 8 bytes before it, the parameters right behind it).  The record is kept on the descriptor: the
+    library reads it while the descriptor is handed over (add_member, stage, consume, ...)."""
+    numel = 1
+    for n in shape:
+        numel *= int(n)
+    inner = 1
+    for n in shape[axis + 1 :]:
+        inner *= int(n)
+    rec = QChannel(channels=int(shape[axis]), inner=inner, body_addr=body, params_addr=body + numel, axis=axis)
+    d.reserved = QSCHEME_PER_CHANNEL
+    d.q_zero_point = C.addressof(rec)
+    d._qchannel = rec
+    return d
+
+
+def rebase(d: CopyDesc, delta: int) -> CopyDesc:
+    """A copy of load descriptor ``d`` whose wire image starts ``delta`` bytes later (a per-channel record moves too)."""
+    c = CopyDesc.from_buffer_copy(d)
+    c.src_addr = d.src_addr + delta
+    if d.reserved == QSCHEME_PER_CHANNEL:
+        r = QChannel.from_buffer_copy(d._qchannel)
+        r.body_addr += delta
+        r.params_addr += delta
+        c.q_zero_point = C.addressof(r)
+        c._qchannel = r
+    return c
+
+
 class EngineConfig(C.Structure):
     _fields_ = [
         ("device", C.c_int32),
@@ -323,10 +369,15 @@ def needs_contiguous_copy(t: torch.Tensor) -> bool:
 _QUANT = {torch.qint8: QINT8, torch.quint8: QUINT8}
 
 
-def save_desc(t: torch.Tensor, wire_offset: int, wire_dtype: Optional[torch.dtype] = None, qparams: Optional[Tuple[float, int]] = None) -> CopyDesc:
+def save_desc(
+    t: torch.Tensor, wire_offset: int, wire_dtype: Optional[torch.dtype] = None, qparams: Optional[Tuple[float, int]] = None,
+    axis: Optional[int] = None,
+) -> CopyDesc:
     """tensor view -> wire image at ``wire_offset`` (C-contiguous layout of ``t.shape``).  ``wire_dtype`` fuses a float
     cast; with ``wire_dtype`` torch.qint8/quint8 and ``qparams=(scale, zero_point)`` the pack kernel quantises and
-    appends the 16-byte per-tensor trailer (T:serialization.py:278-310)."""
+    appends the 16-byte per-tensor trailer (T:serialization.py:278-310).  With ``axis`` instead of ``qparams`` the engine
+    quantises per channel along ``axis`` (non-negative): ``wire_offset`` is then where the int body starts, behind the
+    8-byte axis header, and the channel parameters follow the body."""
     d = CopyDesc()
     sizes, strides = list(t.shape), list(t.stride())
     if len(sizes) > MAX_DIMS:
@@ -342,10 +393,13 @@ def save_desc(t: torch.Tensor, wire_offset: int, wire_dtype: Optional[torch.dtyp
     d.dst_addr = wire_offset
     d.src_dtype = tsnap_dtype(t.dtype)
     if wire_dtype in _QUANT:
-        if qparams is None:
-            raise NativeError(-1, "quantising descriptors need qparams=(scale, zero_point)")
         d.dst_dtype = _QUANT[wire_dtype]
-        d.q_scale, d.q_zero_point = float(qparams[0]), int(qparams[1])
+        if axis is not None:
+            per_channel(d, list(t.shape), axis, wire_offset)
+        elif qparams is not None:
+            d.q_scale, d.q_zero_point = float(qparams[0]), int(qparams[1])
+        else:
+            raise NativeError(-1, "quantising descriptors need qparams=(scale, zero_point) or an axis")
     else:
         d.dst_dtype = tsnap_dtype(wire_dtype or t.dtype)
     d.src_space = _space_of(t)
@@ -375,7 +429,7 @@ def load_desc(
         d.dst_strides[i] = ds
     d.src_addr = wire_offset
     d.dst_addr = t.data_ptr()
-    d.src_dtype = tsnap_dtype(wire_dtype or t.dtype)
+    d.src_dtype = _QUANT[wire_dtype] if wire_dtype in _QUANT else tsnap_dtype(wire_dtype or t.dtype)
     d.dst_dtype = tsnap_dtype(t.dtype)
     d.src_space = SPACE_WIRE
     d.dst_space = _space_of(t)

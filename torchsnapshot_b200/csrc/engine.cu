@@ -613,6 +613,16 @@ static int plan_wave(tsnap_job* job, Wave& w) {
                 const uint64_t nt = tile_count(m);
                 if (nt == 0) continue;
                 const uint32_t mi = uint32_t(w.members.size());
+                if (m.mode == kModeQChannel) {
+                    // a save runs statistics over the same tiles and finalises the parameters before the quantising pack
+                    m.q_zero_point = int64_t(w.qch.size());
+                    w.qch.push_back(nc.qc);
+                    if (nc.qc.save) {
+                        for (uint64_t t = 0; t < nt; ++t) w.tiles[kKernelQStats].push_back(Tile{mi, uint32_t(t)});
+                        for (uint64_t t = 0; t * kQChannelsPerTile < nc.qc.channels; ++t) w.tiles[kKernelQParams].push_back(Tile{mi, uint32_t(t)});
+                        w.qkey_bytes += 16 * nc.qc.channels;
+                    }
+                }
                 w.members.push_back(m);
                 const Kernel kernel = kernel_of(m.mode);
                 *tiles_of[bucket_of(kernel)] += nt;
@@ -632,15 +642,19 @@ static int launch_wave(tsnap_job* job, Wave& w) {
         const void* host;
         size_t bytes, off;
     };
-    Segment seg[2 + kKernelCount];
+    // (then the per-channel parameter table and the key slots of its saves, which are zeroed on the device)
+    Segment seg[3 + kKernelCount];
     seg[0] = {w.members.data(), w.members.size() * sizeof(Member), 0};
     seg[1] = {w.tmaps.data(), w.tmaps.size() * sizeof(TmaPair), 0};
     for (int k = 0; k < kKernelCount; ++k) seg[2 + k] = {w.tiles[k].data(), w.tiles[k].size() * sizeof(Tile), 0};
+    seg[2 + kKernelCount] = {w.qch.data(), w.qch.size() * sizeof(QChannel), 0};
     w.table_bytes = 0;
     for (Segment& s : seg) {
         s.off = w.table_bytes;
         w.table_bytes += align_up(s.bytes, 256);
     }
+    const uint64_t qkeys_off = w.table_bytes;
+    w.table_bytes += w.qkey_bytes;
     for (cudaEvent_t& ev : w.ev_bucket) CUDA_TRY(cudaEventCreate(&ev));
     CUDA_TRY(cudaEventCreateWithFlags(&w.ev_done, cudaEventDisableTiming));
     if (w.members.empty()) {
@@ -651,6 +665,19 @@ static int launch_wave(tsnap_job* job, Wave& w) {
     w.d_tables = eng->get_table(w.table_bytes, &w.table_cap);  // returned to the pool when the job is destroyed
     if (!w.d_tables) return set_err(TSNAP_ECUDA, "out of device memory for the launch tables");
     char* d = static_cast<char*>(w.d_tables);
+    if (w.qkey_bytes) {
+        uint64_t off = qkeys_off;
+        for (QChannel& q : w.qch) {
+            if (!q.save) continue;
+            q.keys = uint64_t(uintptr_t(d + off));
+            off += 16 * q.channels;
+        }
+        if (!job->qflag) {
+            CUDA_TRY(cudaHostAlloc(reinterpret_cast<void**>(&job->qflag), sizeof(int), cudaHostAllocMapped));
+            *job->qflag = 0;
+        }
+        CUDA_TRY(cudaMemsetAsync(d + qkeys_off, 0, w.qkey_bytes, eng->s_kernel));
+    }
     // pageable sources: the runtime stages them before returning, so the vectors may be freed later
     for (const Segment& s : seg) {
         if (s.bytes) CUDA_TRY(cudaMemcpyAsync(d + s.off, s.host, s.bytes, cudaMemcpyHostToDevice, eng->s_kernel));
@@ -658,13 +685,19 @@ static int launch_wave(tsnap_job* job, Wave& w) {
     }
     const Member* d_members = reinterpret_cast<const Member*>(d + seg[0].off);
     const TmaPair* d_maps = reinterpret_cast<const TmaPair*>(d + seg[1].off);
+    const QChannel* d_qch = reinterpret_cast<const QChannel*>(d + seg[2 + kKernelCount].off);
+    int* d_qflag = nullptr;
+    if (job->qflag) CUDA_TRY(cudaHostGetDevicePointer(reinterpret_cast<void**>(&d_qflag), job->qflag, 0));
     // the kernels of a bucket are adjacent in Kernel order: an event closes every bucket, empty or not
     int launched = 0;
     CUDA_TRY(cudaEventRecord(w.ev_bucket[0], eng->s_kernel));
     for (int k = 0; k < kKernelCount; ++k) {
         const Kernel kernel = Kernel(k);
         const Tile* d_tiles = reinterpret_cast<const Tile*>(d + seg[2 + k].off);
-        CUDA_TRY(launch_kernel(kernel, d_members, d_tiles, d_maps, uint32_t(w.tiles[k].size()), eng->sm_count, eng->s_kernel));
+        if (kernel == kKernelQStats || kernel == kKernelQParams || kernel == kKernelQChannel)
+            CUDA_TRY(launch_qchannel_kernel(kernel, d_members, d_qch, d_tiles, uint32_t(w.tiles[k].size()), d_qflag, eng->sm_count, eng->s_kernel));
+        else
+            CUDA_TRY(launch_kernel(kernel, d_members, d_tiles, d_maps, uint32_t(w.tiles[k].size()), eng->sm_count, eng->s_kernel));
         launched += w.tiles[k].empty() ? 0 : 1;
         if (k + 1 == kKernelCount || bucket_of(Kernel(k + 1)) != bucket_of(kernel))
             CUDA_TRY(cudaEventRecord(w.ev_bucket[bucket_of(kernel) + 1], eng->s_kernel));
@@ -1036,12 +1069,12 @@ static void post_host_file(tsnap_job* job, int fi, bool save) {
                 for (size_t i = 0; ok && i < f.members.size(); ++i) {
                     NormalizedCopy nc;
                     int rc = normalize_copy(f.members[i], uint64_t(uintptr_t(tmp)), false, &nc, &err);
+                    if (rc == TSNAP_OK) rc = host_copy_all(nc, &err);
                     if (rc != TSNAP_OK) {
                         job->fail(rc, "member of " + f.path + ": " + err);
                         ok = false;
                         break;
                     }
-                    for (int k = 0; k < nc.n; ++k) host_copy_range(nc.m[k], 0, nc.m[k].bytes);
                 }
                 if (ok && save && pwrite_all(f.fd, tmp, f.nbytes, 0) != 0)
                     job->fail(TSNAP_EIO, "pwrite " + f.path + ": " + strerror(errno));
@@ -1053,6 +1086,12 @@ static void post_host_file(tsnap_job* job, int fi, bool save) {
 }
 
 // ---- save ------------------------------------------------------------------------------------------------
+// after a wave's kernels: did the parameter kernel meet a NaN / Inf channel?
+static void check_nonfinite(tsnap_job* job) {
+    if (job->qflag && *static_cast<volatile int*>(job->qflag))
+        job->fail(TSNAP_EINVAL, "per-channel quantisation: a channel of a source tensor holds a NaN or Inf");
+}
+
 static void mark_device_done(tsnap_job* job) {
     std::lock_guard<std::mutex> g(job->mu);
     if (!job->device_done) {
@@ -1156,10 +1195,13 @@ static int run_save_inner(tsnap_job* job) {
 
     // Sources are reusable (the async_take gate) once the last pack kernel has finished and, when files are drained
     // straight from the live tensors, once the last of those copies has finished.
+    // (a wave that quantises per channel is always armed: its entry fails the job before any chunk of the wave is
+    // written when a channel held a NaN or Inf — the completion thread retires entries in order)
     auto arm_kernel_done = [&](Wave& w, size_t wi, bool gate) {
         Wave* wp = &w;
         push_pending(eng, w.ev_done, [job, wp, wi, gate, eng](bool ok) {
             if (!ok) job->fail(TSNAP_ECUDA, "pack kernel failed");
+            check_nonfinite(job);
             if (eng->trace) {
                 collect_wave_timing(job, *wp);
                 const double t1 = job->now_ms();
@@ -1170,7 +1212,7 @@ static int run_save_inner(tsnap_job* job) {
     };
     for (size_t wi = 0; wi < launched; ++wi) {
         const bool gate = !has_direct && wi + 1 == ns;
-        if (gate || eng->trace) arm_kernel_done(job->waves[wi], wi, gate);
+        if (gate || eng->trace || job->waves[wi].qkey_bytes) arm_kernel_done(job->waves[wi], wi, gate);
     }
     auto launch_next = [&]() -> int {
         Wave& w = job->waves[launched];
@@ -1178,7 +1220,7 @@ static int run_save_inner(tsnap_job* job) {
         int r = launch_wave(job, w);
         if (r != TSNAP_OK) return r;
         const bool gate = !has_direct && launched + 1 == ns;
-        if (gate || eng->trace) arm_kernel_done(w, launched, gate);
+        if (gate || eng->trace || w.qkey_bytes) arm_kernel_done(w, launched, gate);
         ++launched;
         return TSNAP_OK;
     };
@@ -1468,8 +1510,8 @@ static int run_stage_inner(tsnap_job* job) {
         if (d.src_space == TSNAP_SPACE_HOST) {
             NormalizedCopy nc;
             int rc = normalize_copy(d, uint64_t(uintptr_t(job->stage_buf)), false, &nc, &err);
+            if (rc == TSNAP_OK) rc = host_copy_all(nc, &err);
             if (rc != TSNAP_OK) return set_err(rc, err);
-            for (int k = 0; k < nc.n; ++k) host_copy_range(nc.m[k], 0, nc.m[k].bytes);
         } else {
             dev.push_back(d);
         }
@@ -1534,6 +1576,7 @@ static int run_stage_inner(tsnap_job* job) {
     if (!w.direct)
         push_pending(eng, w.ev_done, [job](bool ok) {
             if (!ok) job->fail(TSNAP_ECUDA, "pack kernel failed");
+            check_nonfinite(job);
             mark_device_done(job);
         });
     push_pending(eng, ev, [eng, job, ev, wp](bool ok) {
@@ -1834,7 +1877,13 @@ static int add_member(tsnap_job* job, int32_t fi, const tsnap_copy_desc* d, bool
     FileSpec& f = job->files[size_t(fi)];
     uint64_t numel = 1;
     for (int i = 0; i < d->ndim; ++i) numel *= uint64_t(d->sizes[i]);
-    if (save) {
+    tsnap_copy_desc own = *d;
+    if (d->reserved == TSNAP_QSCHEME_PER_CHANNEL) {
+        // the engine plans after this call returns: keep its own copy of the record
+        if (nc.qc.params + 16 * nc.qc.channels > f.nbytes) return set_err(TSNAP_EINVAL, "per-channel parameters exceed the file's wire image");
+        job->qrecs.push_back(*reinterpret_cast<const tsnap_qchannel*>(uintptr_t(d->q_zero_point)));
+        own.q_zero_point = int64_t(uintptr_t(&job->qrecs.back()));
+    } else if (save) {
         const bool quant = d->dst_dtype == TSNAP_QINT8 || d->dst_dtype == TSNAP_QUINT8;
         const uint64_t end = d->dst_addr + numel * dtype_size(d->dst_dtype) + (quant && numel ? 16 : 0);
         if (end > f.nbytes) return set_err(TSNAP_EINVAL, "member exceeds the file's wire image");
@@ -1853,7 +1902,7 @@ static int add_member(tsnap_job* job, int32_t fi, const tsnap_copy_desc* d, bool
         else
             f.dense = false;
     }
-    f.members.push_back(*d);
+    f.members.push_back(own);
     job->stats.n_members++;
     return TSNAP_OK;
 }
@@ -2000,6 +2049,7 @@ int tsnap_job_destroy(tsnap_job* job) {
     if (job->ev_consumer) cudaEventDestroy(job->ev_consumer);
     if (job->ev_copy_begin) cudaEventDestroy(job->ev_copy_begin);
     if (job->ev_copy_end) cudaEventDestroy(job->ev_copy_end);
+    if (job->qflag) cudaFreeHost(job->qflag);
     for (FileSpec& f : job->files)
         if (f.fd >= 0) close(f.fd);
     delete job;
@@ -2260,8 +2310,11 @@ int tsnap_consume(tsnap_engine* eng, const void* host_buf, uint64_t nbytes, cons
         if (members[i].dst_space == TSNAP_SPACE_HOST) {
             NormalizedCopy nc;
             int rc = normalize_copy(members[i], uint64_t(uintptr_t(host_buf)), false, &nc, &err);
+            if (rc == TSNAP_OK && members[i].reserved == TSNAP_QSCHEME_PER_CHANNEL &&
+                nc.qc.params - uint64_t(uintptr_t(host_buf)) + 16 * nc.qc.channels > nbytes)
+                return set_err(TSNAP_EINVAL, "per-channel parameters exceed the buffer");
+            if (rc == TSNAP_OK) rc = host_copy_all(nc, &err);
             if (rc != TSNAP_OK) return set_err(rc, err);
-            for (int k = 0; k < nc.n; ++k) host_copy_range(nc.m[k], 0, nc.m[k].bytes);
         } else {
             dev.push_back(members[i]);
         }
@@ -2396,6 +2449,14 @@ int tsnap_host_execute(const tsnap_copy_desc* members, int32_t n, void* wire_buf
         NormalizedCopy nc;
         int rc = normalize_copy(d, uint64_t(uintptr_t(wire_buf)), false, &nc, &err);
         if (rc != TSNAP_OK) return set_err(rc, err);
+        if (d.reserved == TSNAP_QSCHEME_PER_CHANNEL) {
+            // three dependent passes over the whole member: one work item, run before the others
+            if (nc.qc.params - uint64_t(uintptr_t(wire_buf)) + 16 * nc.qc.channels > wire_nbytes)
+                return set_err(TSNAP_EINVAL, "per-channel member exceeds the wire buffer");
+            rc = host_copy_all(nc, &err);
+            if (rc != TSNAP_OK) return set_err(rc, err);
+            continue;
+        }
         for (int k = 0; k < nc.n; ++k) {
             const Member& m = nc.m[k];
             const uint64_t wire_off = (d.dst_space == TSNAP_SPACE_WIRE ? m.dst : m.src) - uint64_t(uintptr_t(wire_buf));

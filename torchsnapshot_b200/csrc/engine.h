@@ -173,6 +173,8 @@ struct Wave {
     std::vector<Member> members;
     std::vector<Tile> tiles[kKernelCount];  // per kernel (kernels.h)
     std::vector<TmaPair> tmaps;  // tensor maps of the tensor-map kernels' members (Member.q_zero_point indexes this table)
+    std::vector<QChannel> qch;   // parameters of the kModeQChannel members (Member.q_zero_point indexes this table)
+    uint64_t qkey_bytes = 0;     // save: the key slots of all qch entries (QChannel.keys, filled in by launch_wave)
     void* d_tables = nullptr;
     size_t table_bytes = 0, table_cap = 0;
     cudaEvent_t ev_bucket[kBucketCount + 1] = {};  // kernel timing: bucket b runs between ev_bucket[b] and ev_bucket[b + 1]
@@ -218,6 +220,10 @@ struct tsnap_job {
     int err_code = 0;
     std::string err_msg;
     std::atomic<int64_t> parts_left{0};
+    // per-channel descriptors: the job's own copies of their tsnap_qchannel records (the caller's are only read during
+    // add_member), and the host-mapped word the parameter kernel raises on a NaN / Inf channel
+    std::deque<tsnap_qchannel> qrecs;
+    int* qflag = nullptr;
     // stager seam (kStage): whole-buffer pinned sink
     void* stage_buf = nullptr;
     size_t stage_cap = 0;

@@ -834,6 +834,397 @@ __global__ void __launch_bounds__(kLsuThreads, kMinBlocks) tsnap_lsu_copy_kernel
 }
 
 // ------------------------------------------------------------------------------------------------
+// per-channel quantisation (kModeQChannel): statistics -> parameters -> quantising pack on save, dequantising
+// scatter on restore.  A tile is a kTileLsu range of the member's destination bytes; a save tile is walked in chunks of
+// 16 elements whose wire bytes are one 16 B-aligned vector (the body starts 8 B into a 256 B-aligned file image, so
+// the first and last chunk of a tile may be shorter).
+// ------------------------------------------------------------------------------------------------
+constexpr uint32_t kQChunk = 16;
+constexpr uint32_t kQSmemChannels = 2048;  // members with at most this many channels aggregate a tile in shared memory
+
+// (row, col) of the member's element walk and the byte offsets of the row on both sides
+struct QWalk {
+    uint64_t row, col;
+    int64_t so, dofs;
+};
+__device__ __forceinline__ void qwalk_at(const Member& m, uint64_t e, QWalk& w) {
+    w.row = e / m.inner;
+    w.col = e - w.row * m.inner;
+    outer_offsets(m, w.row, &w.so, &w.dofs);
+}
+__device__ __forceinline__ bool qwalk_next(const Member& m, QWalk& w) {  // true when a new row starts
+    if (++w.col < m.inner) return false;
+    w.col = 0;
+    ++w.row;
+    outer_offsets(m, w.row, &w.so, &w.dofs);
+    return true;
+}
+// channel of the wire byte at `a`, and its position inside the channel's run of `inner` elements
+__device__ __forceinline__ void qchan_at(const QChannel& q, uint64_t a, uint64_t* c, uint64_t* r) {
+    const uint64_t off = a - q.body;
+    if (((off | q.inner | q.channels) >> 32) == 0) {  // 32-bit division: every piece below 4 GiB
+        const uint32_t t = (uint32_t)off / (uint32_t)q.inner;
+        *r = (uint32_t)off - t * (uint32_t)q.inner;
+        *c = t % (uint32_t)q.channels;
+        return;
+    }
+    const uint64_t t = off / q.inner;
+    *r = off - t * q.inner;
+    *c = t % q.channels;
+}
+__device__ __forceinline__ void qchan_next(const QChannel& q, uint64_t* c, uint64_t* r) {
+    if (++*r < q.inner) return;
+    *r = 0;
+    if (++*c == q.channels) *c = 0;
+}
+__device__ __forceinline__ uint64_t ld_u64_any(const char* p) {
+    if ((reinterpret_cast<uintptr_t>(p) & 7) == 0) return *reinterpret_cast<const uint64_t*>(p);
+    uint64_t v = 0;
+    for (int i = 7; i >= 0; --i) v = (v << 8) | (uint8_t)p[i];
+    return v;
+}
+__device__ __forceinline__ void st_u64_any(char* p, uint64_t v) {
+    if ((reinterpret_cast<uintptr_t>(p) & 7) == 0) {
+        *reinterpret_cast<uint64_t*>(p) = v;
+        return;
+    }
+    for (int i = 0; i < 8; ++i) p[i] = (char)(v >> (8 * i));
+}
+
+__device__ __forceinline__ void st_bytes_any(char* p, uint32_t v, int n) {
+    for (int i = 0; i < n; ++i) p[i] = (char)(v >> (8 * i));
+}
+
+// The source elements of save chunk [e, e + n) as fp32 (the value the quantiser reads); 16 B loads when the chunk is
+// a full, 16 B-aligned piece of one dense run.
+__device__ __forceinline__ void qload_chunk(const Member& m, uint64_t e, uint32_t n, float (&x)[kQChunk]) {
+    const char* sb = reinterpret_cast<const char*>(m.src);
+    if (m.nouter == 0 && n == kQChunk && ((m.src + e * m.src_esz) & 15) == 0 && m.src_dtype != TSNAP_F64) {
+        const uint4* p = reinterpret_cast<const uint4*>(sb + e * m.src_esz);
+        if (m.src_dtype == TSNAP_F32) {
+#pragma unroll
+            for (int v = 0; v < 4; ++v) {
+                const uint4 a = ld_stream16(p + v);
+                x[4 * v] = __uint_as_float(a.x);
+                x[4 * v + 1] = __uint_as_float(a.y);
+                x[4 * v + 2] = __uint_as_float(a.z);
+                x[4 * v + 3] = __uint_as_float(a.w);
+            }
+        } else {
+#pragma unroll
+            for (int v = 0; v < 2; ++v) {
+                const uint4 a = ld_stream16(p + v);
+                const uint32_t w[4] = {a.x, a.y, a.z, a.w};
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    const float2 f = m.src_dtype == TSNAP_BF16 ? __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&w[i]))
+                                                               : __half22float2(*reinterpret_cast<const __half2*>(&w[i]));
+                    x[8 * v + 2 * i] = f.x;
+                    x[8 * v + 2 * i + 1] = f.y;
+                }
+            }
+        }
+        return;
+    }
+    QWalk w;
+    qwalk_at(m, e, w);
+#pragma unroll
+    for (uint32_t i = 0; i < kQChunk; ++i) {
+        if (i < n) {
+            x[i] = (float)load_elem(sb + w.so + w.col * m.src_esz, m.src_dtype);
+            qwalk_next(m, w);
+        }
+    }
+}
+
+// chunk k of a save tile [e0, e1): elements [*ce, *ce + *cn), cut at the 16 B boundaries of the wire bytes
+__device__ __forceinline__ bool qsave_chunk(const Member& m, uint64_t e0, uint64_t e1, uint64_t k, uint64_t* ce, uint32_t* cn) {
+    const uint64_t a0 = m.dst + e0, first = (a0 & ~uint64_t(15)) + 16 * k;
+    const uint64_t lo = first > a0 ? first : a0;
+    uint64_t hi = first + 16;
+    if (hi > m.dst + e1) hi = m.dst + e1;
+    if (lo >= hi) return false;
+    *ce = lo - m.dst;
+    *cn = (uint32_t)(hi - lo);
+    return true;
+}
+
+// one run of equal channel: fold (kmin, kmax) into the shared table or the member's key slots.  Lanes holding the same
+// channel are combined first (all 32 lanes call this together; a lane with nothing to add passes c = ~0).
+__device__ __forceinline__ void qstats_flush(uint64_t c, int32_t kmin, int32_t kmax, int* smem, int* keys) {
+    const unsigned peers = __match_any_sync(0xffffffffu, c);
+    const int mn = __reduce_min_sync(peers, kmin), mx = __reduce_max_sync(peers, kmax);
+    if (c != ~uint64_t(0) && (threadIdx.x & 31) == (unsigned)(__ffs(peers) - 1)) {
+        int* slot = smem ? smem + 2 * c : keys + 2 * c;
+        if (mn < 0) atomicMin(slot, mn);
+        if (mx > 0) atomicMax(slot + 1, mx);
+    }
+}
+
+__global__ void __launch_bounds__(kLsuThreads) tsnap_qstats_kernel(const Member* __restrict__ members, const QChannel* __restrict__ qch,
+                                                                   const Tile* __restrict__ tiles, uint32_t ntiles) {
+    __shared__ int table[2 * kQSmemChannels];
+    __shared__ int pacc[2 * kQChunk * kLsuThreads];  // per thread: (min, max) of its 16 chunk positions, see `periodic`
+    for (uint32_t i = threadIdx.x; i < 2 * kQSmemChannels; i += kLsuThreads) table[i] = 0;
+    int* const pmin = pacc + threadIdx.x;                        // position i at pmin[i * kLsuThreads]
+    int* const pmax = pacc + kQChunk * kLsuThreads + threadIdx.x;
+    for (uint32_t t = blockIdx.x; t < ntiles; t += gridDim.x) {
+        const Tile tl = tiles[t];
+        const Member& m = members[tl.member];
+        const QChannel q = qch[m.q_zero_point];
+        const uint64_t lo = (uint64_t)tl.index * kTileLsu, hi = lo + kTileLsu < m.bytes ? lo + kTileLsu : m.bytes;
+        const bool shared = q.channels <= kQSmemChannels;
+        int* keys = reinterpret_cast<int*>(q.keys);
+        __syncthreads();  // the table is clean
+        // every lane runs the same number of iterations so that qstats_flush is called by whole warps
+        const uint64_t nchunks = (((m.dst + hi + 15) & ~uint64_t(15)) - ((m.dst + lo) & ~uint64_t(15))) / 16;
+        const uint64_t iters = (nchunks + kLsuThreads - 1) / kLsuThreads;
+        // When channels x inner divides the stride between a thread's chunks (16 x kLsuThreads wire bytes), every full
+        // chunk of the thread covers the same 16 channel positions: they are accumulated in the thread's own shared-memory
+        // slots, without atomics (axis -1 of a [N, 1024] weight would otherwise cost two atomics per element).  Shared
+        // rather than registers: 32 more registers would cost a resident CTA per SM on every member.
+        const bool periodic = (kQChunk * kLsuThreads) % (q.channels * q.inner) == 0;
+        uint64_t pbase = ~uint64_t(0);  // wire address of this thread's full chunks, modulo the period
+#pragma unroll
+        for (uint32_t i = 0; i < kQChunk; ++i) pmin[i * kLsuThreads] = pmax[i * kLsuThreads] = 0;
+        for (uint64_t it = 0; it < iters; ++it) {
+            uint64_t ce = 0, c = ~uint64_t(0), r = 0;
+            uint32_t cn = 0;
+            int32_t kmin = 0, kmax = 0;
+            if (qsave_chunk(m, lo, hi, it * kLsuThreads + threadIdx.x, &ce, &cn)) {
+                float x[kQChunk];
+                qload_chunk(m, ce, cn, x);
+                if (periodic && cn == kQChunk && ((m.dst + ce) & 15) == 0) {
+                    pbase = m.dst + ce;
+#pragma unroll
+                    for (uint32_t i = 0; i < kQChunk; ++i) {
+                        const int32_t k = qkey(x[i]);
+                        pmin[i * kLsuThreads] = min(pmin[i * kLsuThreads], k);
+                        pmax[i * kLsuThreads] = max(pmax[i * kLsuThreads], k);
+                    }
+                    cn = 0;  // nothing left for the run-by-run path below
+                }
+                if (cn) qchan_at(q, m.dst + ce, &c, &r);
+#pragma unroll
+                for (uint32_t i = 0; i < kQChunk; ++i) {
+                    if (i < cn) {
+                        const int32_t k = qkey(x[i]);
+                        kmin = min(kmin, k);
+                        kmax = max(kmax, k);
+                        if (i + 1 < cn && r + 1 == q.inner) {  // the next element starts another channel: this run is complete
+                            int* slot = shared ? table + 2 * c : keys + 2 * c;
+                            if (kmin < 0) atomicMin(slot, kmin);
+                            if (kmax > 0) atomicMax(slot + 1, kmax);
+                            kmin = kmax = 0;
+                        }
+                        qchan_next(q, &c, &r);
+                    }
+                }
+                // qchan_next moved past the last element: step back to the channel of the pending run
+                if (cn) c = (r == 0 ? (c == 0 ? q.channels - 1 : c - 1) : c);
+            }
+            if (__any_sync(0xffffffffu, c != ~uint64_t(0))) qstats_flush(c, kmin, kmax, shared ? table : nullptr, keys);
+        }
+        if (pbase != ~uint64_t(0)) {
+            uint64_t c, r;
+            qchan_at(q, pbase, &c, &r);
+            for (uint32_t i = 0; i < kQChunk; ++i) {
+                int* slot = shared ? table + 2 * c : keys + 2 * c;
+                if (pmin[i * kLsuThreads] < 0) atomicMin(slot, pmin[i * kLsuThreads]);
+                if (pmax[i * kLsuThreads] > 0) atomicMax(slot + 1, pmax[i * kLsuThreads]);
+                qchan_next(q, &c, &r);
+            }
+        }
+        if (shared) {
+            __syncthreads();
+            // channels the tile touched: one contiguous range of the wire modulo C
+            const uint64_t c_lo = (m.dst + lo - q.body) / q.inner, c_hi = (m.dst + hi - 1 - q.body) / q.inner;
+            const uint64_t span = c_hi - c_lo + 1 < q.channels ? c_hi - c_lo + 1 : q.channels;
+            for (uint64_t j = threadIdx.x; j < span; j += kLsuThreads) {
+                const uint64_t c = (c_lo + j) % q.channels;
+                const int mn = table[2 * c], mx = table[2 * c + 1];
+                if (mn < 0) atomicMin(keys + 2 * c, mn);
+                if (mx > 0) atomicMax(keys + 2 * c + 1, mx);
+                table[2 * c] = table[2 * c + 1] = 0;
+            }
+        }
+    }
+}
+
+// finalises each channel's keys into (scale: f64, zero_point: i64) in place, copies them into the wire image and writes
+// the axis header; a NaN / Inf channel raises *nonfinite
+__global__ void __launch_bounds__(kLsuThreads) tsnap_qparams_kernel(const Member* __restrict__ members, const QChannel* __restrict__ qch,
+                                                                    const Tile* __restrict__ tiles, uint32_t ntiles, int* nonfinite) {
+    for (uint32_t t = blockIdx.x; t < ntiles; t += gridDim.x) {
+        const Tile tl = tiles[t];
+        const Member& m = members[tl.member];
+        const QChannel q = qch[m.q_zero_point];
+        const bool is_signed = m.dst_dtype == TSNAP_QINT8;
+        const uint64_t c0 = (uint64_t)tl.index * kQChannelsPerTile;
+        const uint64_t c1 = c0 + kQChannelsPerTile < q.channels ? c0 + kQChannelsPerTile : q.channels;
+        char* params = reinterpret_cast<char*>(q.params);
+        for (uint64_t c = c0 + threadIdx.x; c < c1; c += kLsuThreads) {
+            int* k = reinterpret_cast<int*>(q.keys) + 2 * c;
+            double scale;
+            int64_t zp;
+            if (!qparams_of(k[0], k[1], is_signed, &scale, &zp)) {
+                *nonfinite = 1;
+                scale = __longlong_as_double(0x7ff8000000000000ll);
+                zp = 0;
+            }
+            // the quantising pack reads (1 / scale: f32, zero_point: i32) per element: 8 B per channel, scales behind them
+            k[0] = __float_as_int((float)(1.0 / scale));
+            k[1] = (int)zp;
+            reinterpret_cast<double*>(q.keys + 8 * q.channels)[c] = scale;
+            st_u64_any(params + 8 * c, (uint64_t)__double_as_longlong(scale));
+            st_u64_any(params + 8 * (q.channels + c), (uint64_t)zp);
+        }
+        if (tl.index == 0 && threadIdx.x == 0) st_u64_any(reinterpret_cast<char*>(q.body) - 8, (uint64_t)q.axis);
+    }
+}
+
+// torch's per-channel quantiser on the device (ATen/native/quantized/cuda/AffineQuantizer.cu): the same rounding as
+// quantize_elem, with the channel's parameters
+__global__ void __launch_bounds__(kLsuThreads) tsnap_qchannel_kernel(const Member* __restrict__ members, const QChannel* __restrict__ qch,
+                                                                     const Tile* __restrict__ tiles, uint32_t ntiles) {
+    for (uint32_t t = blockIdx.x; t < ntiles; t += gridDim.x) {
+        const Tile tl = tiles[t];
+        const Member& m = members[tl.member];
+        const QChannel q = qch[m.q_zero_point];
+        const uint64_t lo = (uint64_t)tl.index * kTileLsu, hi = lo + kTileLsu < m.bytes ? lo + kTileLsu : m.bytes;
+        if (q.save) {
+            const bool is_signed = m.dst_dtype == TSNAP_QINT8;
+            const uint2* kp = reinterpret_cast<const uint2*>(q.keys);                       // (1 / scale: f32, zero_point: i32)
+            const double* scales = reinterpret_cast<const double*>(q.keys + 8 * q.channels);
+            char* db = reinterpret_cast<char*>(m.dst);
+            uint64_t ce;
+            uint32_t cn;
+            for (uint64_t k = threadIdx.x; qsave_chunk(m, lo, hi, k, &ce, &cn); k += kLsuThreads) {
+                float x[kQChunk];
+                qload_chunk(m, ce, cn, x);
+                uint64_t c, r;
+                qchan_at(q, m.dst + ce, &c, &r);
+                uint64_t loaded = ~uint64_t(0);
+                float inv = 1.0f;
+                int zp = 0;
+                uint32_t o[4] = {0, 0, 0, 0};
+#pragma unroll
+                for (uint32_t i = 0; i < kQChunk; ++i) {
+                    if (i < cn) {
+                        if (c != loaded) {
+                            const uint2 p = kp[c];
+                            inv = __uint_as_float(p.x);
+                            zp = (int)p.y;
+                            loaded = c;
+                        }
+                        // nearbyint(x / scale) without a division: x * fp32(1 / scale) is within 3e-5 of the quotient
+                        // (|x / scale| <= 255 under the default rule), so its rounding is the quotient's unless it lies
+                        // that close to a tie — then the division decides, as quantize_elem does it
+                        const float y = x[i] * inv;
+                        const float t = rintf(y);
+                        int v = fabsf(fabsf(y - t) - 0.5f) > 1e-4f && isfinite(y) ? (int)t : (int)nearbyint((double)x[i] / scales[c]);
+                        v += zp;
+                        const int qlo = is_signed ? -128 : 0, qhi = is_signed ? 127 : 255;
+                        v = v < qlo ? qlo : (v > qhi ? qhi : v);
+                        o[i >> 2] |= (uint32_t)(uint8_t)(int8_t)v << (8 * (i & 3));
+                        qchan_next(q, &c, &r);
+                    }
+                }
+                if (cn == kQChunk) {
+                    st_stream16(db + ce, make_uint4(o[0], o[1], o[2], o[3]));  // the wire side of a save is dense
+                } else {
+                    for (uint32_t i = 0; i < cn; ++i) db[ce + i] = (char)(o[i >> 2] >> (8 * (i & 3)));
+                }
+            }
+            continue;
+        }
+        // restore: float((q - zero_point) * scale) in double, converted to the destination dtype
+        const bool is_signed = m.src_dtype == TSNAP_QINT8;
+        const char* sb = reinterpret_cast<const char*>(m.src);
+        char* db = reinterpret_cast<char*>(m.dst);
+        const char* params = reinterpret_cast<const char*>(q.params);
+        bool aligned = (m.dst % m.dst_esz) == 0;
+        for (uint32_t i = 0; i < m.nouter; ++i) aligned = aligned && ((uint64_t)m.dstride[i] % m.dst_esz) == 0;
+        const uint64_t e0 = lo / m.dst_esz, e1 = hi / m.dst_esz;
+        if (m.nouter == 0 && m.dst_dtype != TSNAP_F64 && ((m.dst + e0 * m.dst_esz) & 15) == 0 && ((m.src + e0) & 3) == 0) {
+            // one dense run on both sides: 4 elements per thread and step, a 4-byte load and one 8 or 16-byte store
+            const uint64_t ngroups = (e1 - e0) / 4;
+            uint64_t loaded = ~uint64_t(0);
+            double scale = 1.0, zp = 0.0;
+            for (uint64_t g = threadIdx.x; g < ngroups; g += kLsuThreads) {
+                const uint64_t e = e0 + 4 * g;
+                const uint32_t w = *reinterpret_cast<const uint32_t*>(sb + e);
+                uint64_t c, r;
+                qchan_at(q, m.src + e, &c, &r);
+                float f[4];
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    if (c != loaded) {
+                        scale = __longlong_as_double((long long)ld_u64_any(params + 8 * c));
+                        zp = (double)(int64_t)ld_u64_any(params + 8 * (q.channels + c));
+                        loaded = c;
+                    }
+                    const uint32_t raw = (w >> (8 * i)) & 255;
+                    const double v = is_signed ? (double)(int8_t)raw : (double)raw;
+                    f[i] = (float)((v - zp) * scale);
+                    qchan_next(q, &c, &r);
+                }
+                char* p = db + e * m.dst_esz;
+                if (m.dst_dtype == TSNAP_F32) {
+                    *reinterpret_cast<float4*>(p) = make_float4(f[0], f[1], f[2], f[3]);
+                } else {
+                    uint16_t h[4];
+#pragma unroll
+                    for (int i = 0; i < 4; ++i)
+                        h[i] = m.dst_dtype == TSNAP_BF16 ? __bfloat16_as_ushort(__float2bfloat16_rn(f[i])) : __half_as_ushort(__float2half_rn(f[i]));
+                    *reinterpret_cast<uint2*>(p) = make_uint2(h[0] | ((uint32_t)h[1] << 16), h[2] | ((uint32_t)h[3] << 16));
+                }
+            }
+            if (threadIdx.x == 0) {  // the ragged tail (< 4 elements)
+                for (uint64_t e = e0 + 4 * ngroups; e < e1; ++e) {
+                    uint64_t c, r;
+                    qchan_at(q, m.src + e, &c, &r);
+                    const uint8_t raw = (uint8_t)sb[e];
+                    const int64_t v = is_signed ? (int64_t)(int8_t)raw : (int64_t)raw;
+                    const float f = (float)((double)(v - (int64_t)ld_u64_any(params + 8 * (q.channels + c))) * __longlong_as_double((long long)ld_u64_any(params + 8 * c)));
+                    char* p = db + e * m.dst_esz;
+                    if (m.dst_dtype == TSNAP_F32) *reinterpret_cast<float*>(p) = f;
+                    else *reinterpret_cast<uint16_t*>(p) = m.dst_dtype == TSNAP_BF16 ? __bfloat16_as_ushort(__float2bfloat16_rn(f)) : __half_as_ushort(__float2half_rn(f));
+                }
+            }
+            continue;
+        }
+        for (uint64_t e = e0 + (uint64_t)threadIdx.x * kQChunk; e < e1; e += (uint64_t)kLsuThreads * kQChunk) {
+            const uint32_t n = e1 - e < kQChunk ? (uint32_t)(e1 - e) : kQChunk;
+            QWalk w;
+            qwalk_at(m, e, w);
+            uint64_t c, r;
+            qchan_at(q, m.src + w.so + w.col, &c, &r);
+            for (uint32_t i = 0; i < n; ++i) {
+                const uint8_t raw = (uint8_t)sb[w.so + w.col];
+                const int64_t v = is_signed ? (int64_t)(int8_t)raw : (int64_t)raw;
+                const double scale = __longlong_as_double((long long)ld_u64_any(params + 8 * c));
+                const int64_t zp = (int64_t)ld_u64_any(params + 8 * (q.channels + c));
+                const float f = (float)((double)(v - zp) * scale);
+                char* p = db + w.dofs + w.col * m.dst_esz;
+                if (m.dst_dtype == TSNAP_F32) {
+                    if (aligned) *reinterpret_cast<float*>(p) = f;
+                    else st_bytes_any(p, __float_as_uint(f), 4);
+                } else if (m.dst_dtype == TSNAP_F64) {
+                    st_u64_any(p, (uint64_t)__double_as_longlong((double)f));
+                } else {
+                    const uint16_t h = m.dst_dtype == TSNAP_BF16 ? __bfloat16_as_ushort(__float2bfloat16_rn(f)) : __half_as_ushort(__float2half_rn(f));
+                    if (aligned) *reinterpret_cast<uint16_t*>(p) = h;
+                    else st_bytes_any(p, h, 2);
+                }
+                if (qwalk_next(m, w)) qchan_at(q, m.src + w.so, &c, &r);
+                else qchan_next(q, &c, &r);
+            }
+        }
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
 // launchers
 // ------------------------------------------------------------------------------------------------
 // Ring geometry of the copy-engine kernels: two 48 KiB stages per one-warp CTA, two CTAs per SM (192 KiB of the
@@ -847,6 +1238,7 @@ constexpr int kRowsSmem = kRingStages * kRingStageBytes + kRingStages * (int)siz
 // resident CTAs per SM of the three builds of the LSU kernel (kKernelLsu, kKernelLsuStrided, kKernelLsuTranspose), from
 // the occupancy calculator: each persistent grid is exactly one wave
 static int g_lsu_ctas_per_sm[3] = {3, 2, 6};
+static int g_qchannel_ctas_per_sm[3] = {2, 2, 2};  // kKernelQStats, kKernelQParams, kKernelQChannel (from the occupancy calculator)
 
 cudaError_t init_kernels() {
     cudaError_t e = cudaFuncSetAttribute(tsnap_bulk_copy_kernel<kRingStages, kRingStageBytes>, cudaFuncAttributeMaxDynamicSharedMemorySize, kBulkSmem);
@@ -857,6 +1249,9 @@ cudaError_t init_kernels() {
         if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, tsnap_lsu_copy_kernel<3>, kLsuThreads, 0) == cudaSuccess && n > 0) g_lsu_ctas_per_sm[0] = n;
         if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, tsnap_lsu_copy_kernel<2>, kLsuThreads, 0) == cudaSuccess && n > 0) g_lsu_ctas_per_sm[1] = n;
         if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, tsnap_lsu_copy_kernel<6>, kLsuThreads, 0) == cudaSuccess && n > 0) g_lsu_ctas_per_sm[2] = n;
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, tsnap_qstats_kernel, kLsuThreads, 0) == cudaSuccess && n > 0) g_qchannel_ctas_per_sm[0] = n;
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, tsnap_qparams_kernel, kLsuThreads, 0) == cudaSuccess && n > 0) g_qchannel_ctas_per_sm[1] = n;
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, tsnap_qchannel_kernel, kLsuThreads, 0) == cudaSuccess && n > 0) g_qchannel_ctas_per_sm[2] = n;
     }
     return e;
 }
@@ -874,6 +1269,19 @@ cudaError_t launch_kernel(Kernel k, const Member* d_members, const Tile* d_tiles
         case kKernelLsuStrided: tsnap_lsu_copy_kernel<2><<<grid, kLsuThreads, 0, stream>>>(d_members, d_tiles, ntiles); break;
         case kKernelLsuTranspose: tsnap_lsu_copy_kernel<6><<<grid, kLsuThreads, 0, stream>>>(d_members, d_tiles, ntiles); break;
         default: tsnap_lsu_copy_kernel<3><<<grid, kLsuThreads, 0, stream>>>(d_members, d_tiles, ntiles); break;
+    }
+    return cudaGetLastError();
+}
+
+cudaError_t launch_qchannel_kernel(Kernel k, const Member* d_members, const QChannel* d_qch, const Tile* d_tiles, uint32_t ntiles,
+                                   int* nonfinite, int sm_count, cudaStream_t stream) {
+    if (ntiles == 0) return cudaSuccess;
+    uint32_t grid = (uint32_t)sm_count * (uint32_t)g_qchannel_ctas_per_sm[k - kKernelQStats];
+    if (grid > ntiles) grid = ntiles;
+    switch (k) {
+        case kKernelQStats: tsnap_qstats_kernel<<<grid, kLsuThreads, 0, stream>>>(d_members, d_qch, d_tiles, ntiles); break;
+        case kKernelQParams: tsnap_qparams_kernel<<<grid, kLsuThreads, 0, stream>>>(d_members, d_qch, d_tiles, ntiles, nonfinite); break;
+        default: tsnap_qchannel_kernel<<<grid, kLsuThreads, 0, stream>>>(d_members, d_qch, d_tiles, ntiles); break;
     }
     return cudaGetLastError();
 }

@@ -11,6 +11,9 @@ enum Kernel {
     kKernelBulk,          // kModeBulk: copy-engine ring over dense runs (kernels.cu)
     kKernelRows,          // kModeRows: one copy-engine request per run (kernels.cu)
     kKernelRowsTma,       // kModeRowsTma: tensor-map boxes of many short runs (transpose_tma.cu)
+    kKernelQStats,        // kModeQChannel saves: per-channel min / max of the source into the wave's key slots
+    kKernelQParams,       // kModeQChannel saves: keys -> (scale, zero_point), the wire image's parameters and axis header
+    kKernelQChannel,      // kModeQChannel: quantising pack (16 B of int8 per thread) / dequantising scatter
     kKernelLsu,           // kModeContig, kModeCast: 3 CTAs/SM, 80 registers: unaligned dense runs 0.76, fp32 -> bf16 casts 0.87
     kKernelLsuStrided,    // kModeStrided: 2 CTAs/SM, 128 registers: the strided gather keeps 8 independent 16 B loads per
                           // thread in flight without spilling (0.68 on 128 B runs)
@@ -32,6 +35,7 @@ inline Kernel kernel_of(uint32_t mode) {
         case kModeStrided: return kKernelLsuStrided;
         case kModeTranspose: return kKernelLsuTranspose;
         case kModeTransposeTma: return kKernelTransposeTma;
+        case kModeQChannel: return kKernelQChannel;
         default: return kKernelLsu;  // kModeContig, kModeCast
     }
 }
@@ -43,6 +47,11 @@ cudaError_t init_kernels();
 // the SM count times the kernel's resident CTAs per SM, capped at the tile count.  d_maps: the wave's tensor maps.
 cudaError_t launch_kernel(Kernel k, const Member* d_members, const Tile* d_tiles, const TmaPair* d_maps, uint32_t ntiles,
                           int sm_count, cudaStream_t stream);
+
+// launch_kernel for the three kModeQChannel kernels: `d_qch` is the wave's QChannel table, `nonfinite` a word the
+// parameter kernel sets when a channel holds a NaN or Inf
+cudaError_t launch_qchannel_kernel(Kernel k, const Member* d_members, const QChannel* d_qch, const Tile* d_tiles, uint32_t ntiles,
+                                   int* nonfinite, int sm_count, cudaStream_t stream);
 
 // transpose_tma.cu.  make_tma_pair encodes the two tensor maps of a kModeTranspose member (false: the member stays on the
 // LSU transpose — 1-byte elements, bases or strides that are not 16 B multiples, more than 3 extra dims,

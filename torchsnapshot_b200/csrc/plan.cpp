@@ -1,5 +1,6 @@
 #include "plan.h"
 
+#include <algorithm>
 #include <cmath>
 #include <cstring>
 
@@ -20,6 +21,9 @@ bool cast_supported(int s, int d) {
     if (s == d) return !is_quant(s);  // quantised wire elements only exist as the product of a quantising save
     return is_float(s) && (is_float(d) || is_quant(d));
 }
+
+// TSNAP_QSCHEME_PER_CHANNEL: float -> quantised on save, and back on restore
+static bool per_channel_supported(int s, int d) { return (is_float(s) && is_quant(d)) || (is_quant(s) && is_float(d)); }
 
 static inline uint64_t lowbit(uint64_t x) { return x & (~x + 1); }
 
@@ -52,11 +56,16 @@ int normalize_copy(const tsnap_copy_desc& d, uint64_t wire_base, bool allow_bulk
     if (d.src_space == TSNAP_SPACE_WIRE && d.dst_space == TSNAP_SPACE_WIRE)
         return fail(TSNAP_EINVAL, "wire-to-wire copies are not a thing");
     const bool cast = d.src_dtype != d.dst_dtype;
-    if (!cast_supported(d.src_dtype, d.dst_dtype))
+    if (d.reserved != TSNAP_QSCHEME_PER_TENSOR && d.reserved != TSNAP_QSCHEME_PER_CHANNEL)
+        return fail(TSNAP_EINVAL, "unknown quantisation scheme in tsnap_copy_desc.reserved");
+    const bool per_channel = d.reserved == TSNAP_QSCHEME_PER_CHANNEL;
+    if (per_channel ? !per_channel_supported(d.src_dtype, d.dst_dtype) : !cast_supported(d.src_dtype, d.dst_dtype))
         return fail(TSNAP_EUNSUP, "unsupported dtype conversion");
     const bool quant = is_quant(d.dst_dtype);
-    if (quant && (d.dst_space != TSNAP_SPACE_WIRE || !(d.q_scale > 0)))
+    if (!per_channel && quant && (d.dst_space != TSNAP_SPACE_WIRE || !(d.q_scale > 0)))
         return fail(TSNAP_EINVAL, "quantising copies need a WIRE destination and q_scale > 0");
+    if (per_channel && (quant ? d.dst_space : d.src_space) != TSNAP_SPACE_WIRE)
+        return fail(TSNAP_EINVAL, "per-channel copies keep the quantised side in WIRE space");
 
     // logical shape; C-contiguous element strides for a WIRE destination
     int64_t cstride[TSNAP_MAX_DIMS];
@@ -70,6 +79,34 @@ int normalize_copy(const tsnap_copy_desc& d, uint64_t wire_base, bool allow_bulk
     }
     uint64_t numel = 1;
     for (int i = 0; i < d.ndim; ++i) numel *= uint64_t(d.sizes[i]);
+    if (per_channel) {
+        // the record is the caller's: read it once, check it against the descriptor, keep absolute addresses
+        if (d.q_zero_point == 0) return fail(TSNAP_EINVAL, "per-channel descriptor without a tsnap_qchannel record");
+        tsnap_qchannel r;
+        std::memcpy(&r, reinterpret_cast<const void*>(uintptr_t(d.q_zero_point)), sizeof(r));
+        if (r.channels <= 0 || r.inner <= 0 || r.channels > (int64_t(1) << 40) || r.inner > (int64_t(1) << 50))
+            return fail(TSNAP_EINVAL, "tsnap_qchannel: channels and inner must be positive");
+        const uint64_t period = uint64_t(r.channels) * uint64_t(r.inner);
+        if (r.params_addr < r.body_addr || (r.params_addr - r.body_addr) % period != 0)
+            return fail(TSNAP_EINVAL, "tsnap_qchannel: the body is not a whole number of channels x inner elements");
+        if (quant) {
+            if (r.body_addr < 8 || d.dst_addr != r.body_addr || r.params_addr != r.body_addr + numel)
+                return fail(TSNAP_EINVAL, "tsnap_qchannel: a per-channel save writes the whole piece: header at body - 8, "
+                                          "body at dst_addr, parameters right behind it");
+            if (r.axis < 0 || r.axis >= d.ndim) return fail(TSNAP_EINVAL, "tsnap_qchannel: axis out of range");
+        } else if (numel) {
+            uint64_t last = d.src_addr;
+            for (int i = 0; i < d.ndim; ++i) last += uint64_t(d.sizes[i] - 1) * uint64_t(d.src_strides[i]);
+            if (d.src_addr < r.body_addr || last >= r.params_addr)
+                return fail(TSNAP_EINVAL, "tsnap_qchannel: the member reads outside the piece's int body");
+        }
+        out->qc.body = r.body_addr + wire_base;
+        out->qc.params = r.params_addr + wire_base;
+        out->qc.channels = uint64_t(r.channels);
+        out->qc.inner = uint64_t(r.inner);
+        out->qc.axis = r.axis;
+        out->qc.save = quant ? 1 : 0;
+    }
     if (numel == 0) return TSNAP_OK;
 
     Dim dims[TSNAP_MAX_DIMS];
@@ -107,7 +144,7 @@ int normalize_copy(const tsnap_copy_desc& d, uint64_t wire_base, bool allow_bulk
     if (cast) {
         m.mode = kModeCast;
         m.unit = uint32_t(ed);
-        if (quant) {
+        if (quant && !per_channel) {
             m.q_scale = d.q_scale;
             m.q_zero_point = d.q_zero_point;
             m.shift = 1;  // append [scale][zero_point] behind the payload
@@ -136,6 +173,10 @@ int normalize_copy(const tsnap_copy_desc& d, uint64_t wire_base, bool allow_bulk
     }
 
     if (cast) {
+        if (per_channel) {
+            m.mode = kModeQChannel;
+            m.shift = 0;
+        }
         out->m[0] = m;
         out->n = 1;
         return TSNAP_OK;
@@ -327,6 +368,80 @@ void host_copy_range(const Member& m, uint64_t lo, uint64_t hi) {
         std::memcpy(dst + m.bytes, &m.q_scale, 8);
         std::memcpy(dst + m.bytes + 8, &m.q_zero_point, 8);
     }
+}
+
+// ---- per-channel quantisation on the host ------------------------------------------------------------------
+static inline void store_float(void* p, uint32_t dt, float f) {
+    switch (dt) {
+        case TSNAP_F16: { _Float16 h = (_Float16)f; std::memcpy(p, &h, 2); break; }
+        case TSNAP_BF16: { uint16_t v = f32_to_bf16(f); std::memcpy(p, &v, 2); break; }
+        case TSNAP_F32: std::memcpy(p, &f, 4); break;
+        default: { double x = double(f); std::memcpy(p, &x, 8); }
+    }
+}
+
+// The three passes of the device (statistics, parameters, quantising pack) in one sequential sweep each, with the same
+// rules: the element as fp32, channel keys that start at 0, the parameters of qparams_of, torch's CPU quantiser.
+int host_qchannel(const Member& m, const QChannel& q, std::string* err) {
+    const char* src = reinterpret_cast<const char*>(uintptr_t(m.src));
+    char* dst = reinterpret_cast<char*>(uintptr_t(m.dst));
+    const uint64_t n = m.bytes / m.dst_esz;
+    char* params = reinterpret_cast<char*>(uintptr_t(q.params));
+    auto channel = [&](uint64_t wire_addr) { return ((wire_addr - q.body) / q.inner) % q.channels; };
+    const bool is_signed = (q.save ? m.dst_dtype : m.src_dtype) == TSNAP_QINT8;
+    if (!q.save) {
+        for (uint64_t e = 0; e < n; ++e) {
+            const uint64_t row = e / m.inner, col = e % m.inner;
+            int64_t so, dofs;
+            outer_offsets(m, row, &so, &dofs);
+            const uint64_t a = m.src + uint64_t(so) + col;
+            const uint64_t c = channel(a);
+            double scale;
+            int64_t zp;
+            std::memcpy(&scale, params + 8 * c, 8);
+            std::memcpy(&zp, params + 8 * (q.channels + c), 8);
+            const uint8_t raw = *reinterpret_cast<const uint8_t*>(uintptr_t(a));
+            const int64_t v = is_signed ? int64_t(int8_t(raw)) : int64_t(raw);
+            store_float(dst + dofs + col * m.dst_esz, m.dst_dtype, float(double(v - zp) * scale));
+        }
+        return TSNAP_OK;
+    }
+    std::vector<int32_t> kmin(q.channels, 0), kmax(q.channels, 0);
+    for (uint64_t e = 0; e < n; ++e) {
+        const uint64_t row = e / m.inner, col = e % m.inner;
+        int64_t so, dofs;
+        outer_offsets(m, row, &so, &dofs);
+        const int32_t k = qkey(float(load_as_double(src + so + col * m.src_esz, m.src_dtype)));
+        const uint64_t c = channel(m.dst + uint64_t(dofs) + col);
+        kmin[c] = std::min(kmin[c], k);
+        kmax[c] = std::max(kmax[c], k);
+    }
+    std::vector<double> scale(q.channels);
+    std::vector<int64_t> zp(q.channels);
+    for (uint64_t c = 0; c < q.channels; ++c) {
+        if (!qparams_of(kmin[c], kmax[c], is_signed, &scale[c], &zp[c])) {
+            if (err) *err = "per-channel quantisation: channel " + std::to_string(c) + " holds a NaN or Inf";
+            return TSNAP_EINVAL;
+        }
+    }
+    std::memcpy(reinterpret_cast<char*>(uintptr_t(q.body)) - 8, &q.axis, 8);
+    std::memcpy(params, scale.data(), 8 * q.channels);
+    std::memcpy(params + 8 * q.channels, zp.data(), 8 * q.channels);
+    for (uint64_t e = 0; e < n; ++e) {
+        const uint64_t row = e / m.inner, col = e % m.inner;
+        int64_t so, dofs;
+        outer_offsets(m, row, &so, &dofs);
+        const float x = float(load_as_double(src + so + col * m.src_esz, m.src_dtype));
+        const uint64_t c = channel(m.dst + uint64_t(dofs) + col);
+        reinterpret_cast<uint8_t*>(dst + dofs)[col] = quantize_host(x, scale[c], zp[c], is_signed);
+    }
+    return TSNAP_OK;
+}
+
+int host_copy_all(const NormalizedCopy& nc, std::string* err) {
+    if (nc.n == 1 && nc.m[0].mode == kModeQChannel) return host_qchannel(nc.m[0], nc.qc, err);
+    for (int k = 0; k < nc.n; ++k) host_copy_range(nc.m[k], 0, nc.m[k].bytes);
+    return TSNAP_OK;
 }
 
 }  // namespace tsnap

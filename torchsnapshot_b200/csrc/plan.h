@@ -8,6 +8,7 @@
 // sides and calls Tensor.copy_ (T:io_preparers/sharded_tensor.py:285-323).  We never materialise the
 // contiguous temporary: the strided gather/scatter IS the copy.
 #pragma once
+#include <cmath>
 #include <cstdint>
 #include <string>
 #include <vector>
@@ -40,10 +41,30 @@ enum Mode : uint32_t {
                             // many runs (rows x run) instead of one copy-engine request per run; chosen per wave by the engine
     kModeRows = 4,     // kModeStrided whose runs, strides and bases are all multiples of 16 B and whose runs are long
                        // enough for the copy engine: one cp.async.bulk per run (or one per stage on a dense side)
+    kModeQChannel = 8,  // kModeCast of a TSNAP_QSCHEME_PER_CHANNEL descriptor: float -> QINT8/QUINT8 (save) or back
+                        // (restore) with per-channel parameters; q_zero_point indexes the wave's QChannel table
 };
 constexpr uint32_t kRowsSrcDense = 1;  // Member.shift bits in kModeRows: consecutive runs are adjacent on that side
 constexpr uint32_t kRowsDstDense = 2;
 constexpr uint64_t kRowsMinRun = 256;  // shorter runs stay on the LSU path (one copy-engine request per run does not pay)
+
+// Per-channel parameters of one kModeQChannel member: absolute addresses in the space the wire image lives in.
+// The channel of the wire element at address a is ((a - body) / inner) % channels.
+struct alignas(16) QChannel {
+    uint64_t body;      // first int element of the piece
+    uint64_t params;    // scales[channels] (f64), then zero_points[channels] (i64)
+    uint64_t channels;
+    uint64_t inner;
+    int64_t axis;
+    uint64_t keys;      // save: 16 B per channel in the launch table, zeroed in stream order before the wave: 8 B per
+                        // channel of running (min, max) keys of the statistics pass, which the parameter pass replaces by
+                        // (1 / scale: f32, zero_point: i32) for the quantising pack, then the scales (f64).  (The wire
+                        // image's parameter area cannot hold them: it follows a body of any length, so it is not even
+                        // 4 B aligned in general.)
+    uint32_t save;      // 1: float -> int (statistics, parameters, header), 0: int -> float
+    uint32_t pad;
+};
+constexpr uint32_t kQChannelsPerTile = 8192;  // channels per tile of the header/parameter kernels
 
 // Device-visible member record.  Addresses are absolute for the space they live in.
 struct alignas(16) Member {
@@ -65,7 +86,8 @@ struct alignas(16) Member {
     int64_t dstride[kMaxOuter];  // bytes
     double q_scale;              // kModeCast to TSNAP_QINT8/QUINT8: affine quantisation parameters; when `shift` bit 0
     int64_t q_zero_point;        // is set the tile holding the last element appends the 16-byte trailer at dst + bytes
-                                 // kModeTransposeTma: index of the member's TmaPair in the wave's tensor-map table
+                                 // kModeTransposeTma: index of the member's TmaPair in the wave's tensor-map table;
+                                 // kModeQChannel: index of its QChannel in the wave's table
 };
 
 // Two CUtensorMap objects (128 B each, 64 B-aligned) of one kModeTransposeTma member, both of rank 5:
@@ -156,6 +178,7 @@ struct NormalizedCopy {
     Member m[2];
     int n = 0;
     int src_space = 0, dst_space = 0;
+    QChannel qc{};  // m[0].mode == kModeQChannel: its parameters (m[0].q_zero_point is set by whoever tables them)
 };
 
 // Normalises one descriptor.  `src_base`/`dst_base` are added to WIRE-space addresses (the absolute
@@ -169,5 +192,52 @@ bool cast_supported(int src_dt, int dst_dt);
 
 // Host execution of one member over logical byte range [lo,hi) (memcpy of runs / scalar casts).
 void host_copy_range(const Member& m, uint64_t lo, uint64_t hi);
+
+// Host execution of a whole kModeQChannel member: on save the statistics, parameters, header and quantised body; on
+// restore the dequantisation.  Returns TSNAP_EINVAL (with `err`) when a saved channel holds a NaN or Inf.
+int host_qchannel(const Member& m, const QChannel& q, std::string* err);
+// Every member of a normalised copy on the host
+int host_copy_all(const NormalizedCopy& nc, std::string* err);
+
+// Ordered-int key of a float (signed comparison of keys == float comparison for non-NaN values), and back.  The
+// statistics pass keeps the running min / max of a channel as two keys; both start at key(0.0f) = 0, so every range
+// includes 0 — exactly what both default rules need.
+TSNAP_HD inline int32_t qkey(float f) {
+    int32_t i;
+#ifdef __CUDA_ARCH__
+    i = __float_as_int(f);
+#else
+    __builtin_memcpy(&i, &f, 4);
+#endif
+    return i >= 0 ? i : i ^ 0x7fffffff;
+}
+TSNAP_HD inline float qkey_value(int32_t k) {
+    const int32_t i = k >= 0 ? k : k ^ 0x7fffffff;
+    float f;
+#ifdef __CUDA_ARCH__
+    f = __int_as_float(i);
+#else
+    __builtin_memcpy(&f, &i, 4);
+#endif
+    return f;
+}
+constexpr int32_t kQKeyMax = 0x7f7fffff;                  // key of FLT_MAX: larger keys are +Inf / NaN
+constexpr int32_t kQKeyMin = int32_t(0xff7fffffu ^ 0x7fffffffu);  // key of -FLT_MAX: smaller keys are -Inf / NaN
+// (scale, zero_point) of one channel from its (min, max) keys, in double as the default rule states; false on NaN / Inf
+TSNAP_HD inline bool qparams_of(int32_t kmin, int32_t kmax, bool is_signed, double* scale, int64_t* zp) {
+    if (kmax > kQKeyMax || kmin < kQKeyMin) return false;
+    const double lo = (double)qkey_value(kmin), hi = (double)qkey_value(kmax);
+    if (is_signed) {
+        const double amax = hi > -lo ? hi : -lo;
+        *scale = amax / 127.0;
+        if (*scale == 0.0) *scale = 1.0;
+        *zp = 0;
+    } else {
+        *scale = (hi - lo) / 255.0;
+        if (*scale == 0.0) *scale = 1.0;
+        *zp = (int64_t)rint(-lo / *scale);  // round half to even (default rounding mode)
+    }
+    return true;
+}
 
 }  // namespace tsnap

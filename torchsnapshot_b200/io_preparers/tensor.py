@@ -12,6 +12,7 @@ from __future__ import annotations
 
 import asyncio
 import math
+import struct
 from concurrent.futures import Executor
 from typing import Any, Callable, List, Optional, Tuple, Union
 
@@ -34,8 +35,8 @@ from ..serialization import (
 
 RAW = Serializer.BUFFER_PROTOCOL.value
 PICKLED = Serializer.TORCH_SAVE.value
-from ..prepare import PER_TENSOR_QTENSOR, fused_quant_of  # noqa: E402
-from ..serialization import per_tensor_qtensor_from_bytes  # noqa: E402
+from ..prepare import PER_CHANNEL_QTENSOR, PER_TENSOR_QTENSOR, PerChannel, fused_quant_of  # noqa: E402
+from ..serialization import per_channel_qtensor_from_bytes, per_tensor_qtensor_from_bytes  # noqa: E402
 PrepareFunc = Callable[[torch.Tensor, bool], torch.Tensor]
 
 
@@ -45,7 +46,17 @@ def entry_nbytes(entry: TensorEntry) -> int:
         n *= s
     if entry.serializer == PER_TENSOR_QTENSOR:
         n += 16  # [q_scale: double][q_zero_point: int64] behind the int_repr bytes (T:serialization.py:278-310)
+    elif entry.serializer == PER_CHANNEL_QTENSOR:
+        n += 8  # the axis header; the 16 B per channel behind the body depend on the axis, which only the file records
     return n
+
+
+def per_channel_wire_nbytes(shape, axis: int) -> int:
+    """Size of a per-channel file: [axis][int_repr bytes][scales: f64 x C][zero_points: i64 x C]."""
+    numel = 1
+    for s in shape:
+        numel *= s
+    return 8 + numel + 16 * shape[axis]
 
 
 def engine_for(t: torch.Tensor) -> "_native.Engine":
@@ -70,8 +81,10 @@ class TensorBufferStager(BufferStager):
         self.entry = entry
         self.is_async_snapshot = is_async_snapshot
         self._tensor_prepare_func = _tensor_prepare_func
-        # (qdtype, scale, zero_point) when the entry is a quantise-on-save one: the pack kernel quantises
-        self.qparams = fused_quant_of(_tensor_prepare_func, tensor) if entry.serializer == PER_TENSOR_QTENSOR else None
+        # (qdtype, scale, zero_point) when the entry is a quantise-on-save one, a PerChannel for a per-channel one: the
+        # pack kernel quantises
+        quantised = entry.serializer in (PER_TENSOR_QTENSOR, PER_CHANNEL_QTENSOR)
+        self.qparams = fused_quant_of(_tensor_prepare_func, tensor) if quantised else None
 
     # ---- engine-facing description ------------------------------------------------------------
     def is_raw(self) -> bool:
@@ -87,6 +100,8 @@ class TensorBufferStager(BufferStager):
         return t
 
     def wire_nbytes(self) -> int:
+        if isinstance(self.qparams, PerChannel):
+            return per_channel_wire_nbytes(list(self.entry.shape), self.qparams.axis)
         return entry_nbytes(self.entry)
 
     def native_descs(self, wire_offset: int) -> Tuple[List["_native.CopyDesc"], List[torch.Tensor]]:
@@ -94,6 +109,11 @@ class TensorBufferStager(BufferStager):
             t = self.tensor.detach()
             if self.is_async_snapshot and t.device.type == "cpu":
                 t = t.clone()
+            if isinstance(self.qparams, PerChannel):
+                if _native.needs_contiguous_copy(t):
+                    t = t.contiguous()
+                d = _native.save_desc(t, wire_offset + 8, wire_dtype=self.qparams.dtype, axis=self.qparams.axis)
+                return [d], [t]
             qdtype, scale, zp = self.qparams
             return [_native.save_desc(t, wire_offset, wire_dtype=qdtype, qparams=(scale, zp))], [t]
         t = self.source()
@@ -159,12 +179,28 @@ class TensorBufferConsumer(BufferConsumer):
             return tensor_from_memoryview(memoryview(buf), dtype=string_to_dtype(entry.dtype), shape=entry.shape)
         if entry.serializer == PER_TENSOR_QTENSOR:
             return per_tensor_qtensor_from_bytes(bytes(buf), string_to_dtype(entry.dtype), list(entry.shape))
+        if entry.serializer == PER_CHANNEL_QTENSOR:
+            return per_channel_qtensor_from_bytes(bytes(buf), string_to_dtype(entry.dtype), list(entry.shape))
         raise ValueError(f"Unrecognized serializer: {entry.serializer}.")
+
+    def per_channel_descs(self, buf) -> Optional[List["_native.CopyDesc"]]:
+        """Dequantising scatter of a per-channel image in ``buf`` into a float target, or None for other entries."""
+        shape = list(self.entry.shape)
+        if self.entry.serializer != PER_CHANNEL_QTENSOR or self.tensor.dtype not in _FLOATS or list(self.tensor.shape) != shape:
+            return None
+        axis = struct.unpack_from("<q", buf, 0)[0] if len(buf) >= 8 else -1
+        if not 0 <= axis < len(shape) or len(buf) != per_channel_wire_nbytes(shape, axis):
+            raise RuntimeError(f"per-channel image of {len(buf)} bytes with axis {axis} does not fit shape {shape}")
+        if self.tensor.numel() == 0:
+            return []
+        qdtype = string_to_dtype(self.entry.dtype)
+        return [_native.per_channel(_native.load_desc(self.tensor.detach(), 8, wire_dtype=qdtype), shape, axis, 8)]
 
     async def consume_buffer(self, buf: bytes, executor: Optional[Executor] = None) -> None:
         def work() -> None:
-            if self.is_raw():
-                descs, _ = self.native_descs(0)
+            quantised = self.per_channel_descs(buf)
+            if self.is_raw() or quantised is not None:
+                descs = quantised if quantised is not None else self.native_descs(0)[0]
                 if descs:
                     engine_for(self.tensor).consume(buf, descs)
             else:
@@ -178,6 +214,20 @@ class TensorBufferConsumer(BufferConsumer):
     def get_consuming_cost_bytes(self) -> int:
         n = entry_nbytes(self.entry)
         return n if self.is_raw() else 2 * n
+
+
+class _DecodingConsumer(BufferConsumer):
+    """Decodes a quantised entry into a new quantised tensor (read without an in-place target)."""
+
+    def __init__(self, entry: TensorEntry, fut: Future) -> None:
+        self.entry = entry
+        self.fut = fut
+
+    async def consume_buffer(self, buf: bytes, executor: Optional[Executor] = None) -> None:
+        self.fut.obj = TensorBufferConsumer.deserialize_tensor(buf, self.entry)
+
+    def get_consuming_cost_bytes(self) -> int:
+        return 2 * entry_nbytes(self.entry)
 
 
 _FLOATS = (torch.float16, torch.bfloat16, torch.float32, torch.float64)
@@ -214,7 +264,10 @@ class TensorIOPreparer:
                 f"(changed from {tensor.shape} to {traced.shape})."
             )
         serializer = RAW if traced.dtype in BUFFER_PROTOCOL_SUPPORTED_DTYPES else PICKLED
-        if _tensor_prepare_func is not None and fused_quant_of(_tensor_prepare_func, tensor) is not None:
+        quant = fused_quant_of(_tensor_prepare_func, tensor) if _tensor_prepare_func is not None else None
+        if isinstance(quant, PerChannel):
+            serializer = PER_CHANNEL_QTENSOR  # axis header + int_repr + per-channel parameters, produced by the engine
+        elif quant is not None:
             serializer = PER_TENSOR_QTENSOR  # int_repr + 16-byte trailer, produced by the pack kernel
         entry = TensorEntry(
             location=storage_path,
@@ -234,7 +287,7 @@ class TensorIOPreparer:
     def can_load_inplace(entry: Union[TensorEntry, ChunkedTensorEntry], obj: Any) -> bool:
         if not isinstance(obj, torch.Tensor) or list(entry.shape) != list(obj.shape):
             return False
-        if getattr(entry, "serializer", None) == PER_TENSOR_QTENSOR and obj.dtype in _FLOATS:
+        if getattr(entry, "serializer", None) in (PER_TENSOR_QTENSOR, PER_CHANNEL_QTENSOR) and obj.dtype in _FLOATS:
             return True  # dequantised into the float tensor it was quantised from (tensor_copy)
         return string_to_dtype(entry.dtype) == obj.dtype
 
@@ -252,6 +305,10 @@ class TensorIOPreparer:
         tensor_out: Optional[torch.Tensor] = None,
         buffer_size_limit_bytes: Optional[int] = None,
     ) -> Tuple[List[ReadReq], Future[torch.Tensor]]:
+        if entry.serializer == PER_CHANNEL_QTENSOR and (tensor_out is None or not cls.can_load_inplace(entry, tensor_out)):
+            # no float target: the result is the decoded quantised tensor
+            fut: Future[torch.Tensor] = Future()
+            return [ReadReq(path=entry.location, byte_range=entry.byte_range_tuple, buffer_consumer=_DecodingConsumer(entry, fut))], fut
         if tensor_out is None or not cls.can_load_inplace(entry, tensor_out):
             tensor_out = cls.empty_tensor_from_entry(entry)
         if buffer_size_limit_bytes is not None and entry.serializer == RAW:

@@ -7,11 +7,14 @@ reference's own ``TensorBufferStager`` / ``BatchedBufferStager`` / ``GPUBatchedB
 which is what lets ``torchsnapshot_b200.install()`` put the engine underneath an unmodified torchsnapshot."""
 from __future__ import annotations
 
+import os
+import struct
 from typing import Any, List, Optional, Tuple
 
 import torch
 
 from . import _native
+from .prepare import PER_CHANNEL_QTENSOR
 from .serialization import BUFFER_PROTOCOL_SUPPORTED_DTYPES
 
 RAW = "buffer_protocol"
@@ -65,9 +68,10 @@ def _describe_tensor_stager(st: Any, offset: int, clones: Optional[HostCloneBudg
     entry = getattr(st, "entry", None)
     tensor = getattr(st, "tensor", None)
     if entry is not None and isinstance(tensor, torch.Tensor) and getattr(st, "qparams", None) is not None:
-        # quantise-on-save: the pack kernel produces int_repr + trailer (prepare.quantize_on_save)
+        # quantise-on-save: the pack kernel produces int_repr + trailer, or the engine the whole per-channel image
+        # (prepare.quantize_on_save)
         descs, keep = st.native_descs(offset)
-        return descs, keep, tensor.numel() + 16
+        return descs, keep, st.wire_nbytes()
     if entry is None or not isinstance(tensor, torch.Tensor) or getattr(entry, "serializer", None) != RAW:
         return None
     if entry.dtype not in _DTYPES:
@@ -116,8 +120,63 @@ def describe_stager(st: Any, clones: Optional[HostCloneBudget] = None) -> Option
 
 
 # ---- restore side ----------------------------------------------------------------------------------
-def _describe_tensor_consumer(c: Any, offset: int) -> Optional[Described]:
+def per_channel_layout(path: str, entry: Any) -> Tuple[int, int]:
+    """(file size, axis) of a per-channel file, from the file itself: the manifest records neither."""
+    from .io_preparers.tensor import per_channel_wire_nbytes
+
+    shape = list(entry.shape)
+    size = os.stat(path).st_size
+    with open(path, "rb") as f:
+        head = f.read(8)
+    axis = struct.unpack("<q", head)[0] if len(head) == 8 else -1
+    if not 0 <= axis < len(shape):
+        raise RuntimeError(f"{path}: per-channel header names axis {axis}, but the saved tensor has shape {shape}")
+    if size != per_channel_wire_nbytes(shape, axis):
+        raise RuntimeError(f"{path}: {size} bytes, but a per-channel image of shape {shape} along axis {axis} has "
+                           f"{per_channel_wire_nbytes(shape, axis)}")
+    return size, axis
+
+
+def _describe_per_channel_consumer(c: Any, offset: int, root: Optional[str]) -> Optional[Described]:
+    """Dequantising scatter of a per-channel entry into float targets (the whole tensor or reshard overlaps)."""
+    entry = c.entry
+    regions = getattr(c, "overlapping_regions", None)
+    targets = [r.dst_tensor for r in regions] if regions is not None else [getattr(c, "tensor", None)]
+    if root is None or getattr(entry, "byte_range", None) is not None or int(getattr(c, "wire_skip", 0) or 0):
+        return None
+    if not all(isinstance(t, torch.Tensor) and t.dtype in _FLOATS for t in targets):
+        return None  # quantised targets keep torch's own copy semantics
+    nbytes, axis = per_channel_layout(os.path.join(root, entry.location), entry)
+    qdtype = {"torch.qint8": torch.qint8, "torch.quint8": torch.quint8}[entry.dtype]
+    shape = list(entry.shape)
+    strides = _native._c_strides(shape)
+    body = offset + 8
+
+    def desc(dst: torch.Tensor, first: int):
+        return _native.per_channel(_native.load_desc(dst, body + first, wire_dtype=qdtype, wire_strides=strides), shape, axis, body)
+
+    if regions is None:
+        dst = c.tensor.detach()
+        if list(dst.shape) != shape:
+            return None
+        return ([desc(dst, 0)] if dst.numel() else []), [dst], nbytes
+    descs, keep = [], []
+    for region in regions:
+        dst = region.dst_tensor.detach()
+        first = 0
+        for dim, so, do, n in region.overlap_region:
+            dst = dst.narrow(dim, do, n)
+            first += so * strides[dim]
+        if dst.numel():
+            descs.append(desc(dst, first))
+            keep.append(region.dst_tensor)
+    return descs, keep, nbytes
+
+
+def _describe_tensor_consumer(c: Any, offset: int, root: Optional[str] = None) -> Optional[Described]:
     entry = getattr(c, "entry", None)
+    if entry is not None and getattr(entry, "serializer", None) == PER_CHANNEL_QTENSOR:
+        return _describe_per_channel_consumer(c, offset, root)
     if entry is None or getattr(entry, "serializer", None) != RAW or entry.dtype not in _DTYPES:
         return None
     src_dtype = _DTYPES[entry.dtype]
@@ -158,7 +217,10 @@ def _describe_tensor_consumer(c: Any, offset: int) -> Optional[Described]:
     return [_native.load_desc(dst, offset, wire_dtype=src_dtype)], [dst], nbytes
 
 
-def describe_consumer(c: Any) -> Optional[Described]:
+def describe_consumer(c: Any, root: Optional[str] = None) -> Optional[Described]:
+    """(descriptors, keep-alive tensors, wire size) of one ReadReq's consumer, or None when it has to go through its own
+    ``consume_buffer``.  ``root``: directory the entries' locations are relative to; per-channel entries need it to read
+    their layout from the file."""
     members = getattr(c, "byte_range_to_buffer_consumer", None)
     if members is not None:
         descs: List[Any] = []
@@ -170,7 +232,7 @@ def describe_consumer(c: Any) -> Optional[Described]:
             descs += one[0]
             keep += one[1]
         return descs, keep, int(getattr(c, "buf_sz_bytes", 0))
-    return _describe_tensor_consumer(c, 0)
+    return _describe_tensor_consumer(c, 0, root)
 
 
 def native_root(storage: Any, op: str = "write") -> Optional[str]:

@@ -67,10 +67,40 @@ def fused_cast_of(func, tensor: torch.Tensor) -> Optional[torch.dtype]:
 
 
 PER_TENSOR_QTENSOR = "per_tensor_qtensor"  # TensorEntry.serializer of the reference's per-tensor format (T:serialization.py:278-310)
+PER_CHANNEL_QTENSOR = "per_channel_qtensor"  # ... and of its per-channel format (T:serialization.py:366-477)
+
+
+class PerChannel:
+    """What a per-channel quantise-on-save hook reports for a tensor: wire dtype and the (non-negative) axis."""
+
+    def __init__(self, dtype: torch.dtype, axis: int) -> None:
+        self.dtype, self.axis = dtype, axis
+
+
+def per_channel_qparams(t: torch.Tensor, dtype: torch.dtype, axis: int) -> "tuple[torch.Tensor, torch.Tensor]":
+    """The default rule of ``quantize_on_save`` per channel, computed by torch: (scales: float64, zero_points: int64)
+    of ``t`` along ``axis``.  The engine computes the same on the device or host while it packs; this is what the
+    ``tracing=False`` path of the hook (and the tests) use."""
+    x = t.detach().float().movedim(axis, 0).reshape(t.shape[axis], -1)
+    if not bool(torch.isfinite(x).all()):
+        raise ValueError("per-channel quantisation: a channel holds a NaN or Inf")
+    lo = x.amin(1).clamp(max=0).double()
+    hi = x.amax(1).clamp(min=0).double()
+    # divisors as tensors: a Python-scalar divisor is applied as a multiplication by its reciprocal on CUDA, which is
+    # not the rule's (correctly rounded) division
+    if dtype == torch.qint8:
+        scale = torch.maximum(hi, -lo) / torch.full_like(hi, 127.0)
+        zp = torch.zeros_like(scale, dtype=torch.int64)
+    else:
+        scale = (hi - lo) / torch.full_like(hi, 255.0)
+    scale = torch.where(scale == 0, torch.ones_like(scale), scale)
+    if dtype == torch.quint8:
+        zp = torch.round(-lo / scale).to(torch.int64)  # round half to even, like Python's round()
+    return scale, zp
 
 
 def quantize_on_save(dtype: torch.dtype = torch.qint8, qparams: Optional[Callable[[str, torch.Tensor], "tuple[float, int]"]] = None,
-                     only: Optional[str] = None) -> Callable[[str, torch.Tensor, bool], torch.Tensor]:
+                     only: Optional[str] = None, axis: Optional[int] = None) -> Callable[[str, torch.Tensor, bool], torch.Tensor]:
     """A ``_custom_tensor_prepare_func`` that stores floating-point tensors per-tensor affine quantised
     (``torch.qint8`` / ``torch.quint8``) in the reference's self-describing per-tensor format — int_repr bytes followed
     by ``[q_scale: double][q_zero_point: int64]`` (T:serialization.py:278-310, specified and unit-tested there but
@@ -79,9 +109,20 @@ def quantize_on_save(dtype: torch.dtype = torch.qint8, qparams: Optional[Callabl
     T:io_preparers/tensor.py:385-409).
 
     ``qparams(logical_path, tensor) -> (scale, zero_point)``; default: symmetric abs-max scaling for qint8
-    (zero_point 0), min/max affine for quint8."""
+    (zero_point 0), min/max affine for quint8.
+
+    ``axis=k`` (negative counts from the end) quantises per channel along ``k`` instead, in the reference's per-channel
+    format ``[axis: int64][int_repr bytes][scales: float64 x C][zero_points: int64 x C]`` (T:serialization.py:366-477),
+    with the default rule applied to each channel.  It applies to floating-point tensors with ``ndim >= 2`` and
+    ``ndim > k`` and at least one element; 1-d tensors (biases, norms) are stored unchanged, since 16 bytes of
+    parameters per channel would outweigh them.  The engine computes the parameters while it packs; a channel
+    holding a NaN or Inf fails the take."""
     if dtype not in (torch.qint8, torch.quint8):
         raise ValueError("quantize_on_save supports torch.qint8 and torch.quint8")
+    if axis is not None:
+        if qparams is not None:
+            raise ValueError("quantize_on_save: axis (per-channel) does not take caller-supplied qparams")
+        return _quantize_per_channel_on_save(dtype, int(axis), only)
     cache: dict = {}
 
     def default_qparams(_path: str, t: torch.Tensor):
@@ -119,8 +160,33 @@ def quantize_on_save(dtype: torch.dtype = torch.qint8, qparams: Optional[Callabl
     return prepare
 
 
+def _quantize_per_channel_on_save(dtype: torch.dtype, axis: int, only: Optional[str]):
+    def applies(logical_path: Optional[str], tensor: torch.Tensor) -> Optional[PerChannel]:
+        if tensor.dtype not in _FLOATS or tensor.is_quantized or tensor.numel() == 0 or tensor.dim() < 2:
+            return None
+        if not -tensor.dim() <= axis < tensor.dim():
+            return None
+        if only is not None and (logical_path is None or not fnmatch.fnmatch(logical_path, only)):
+            return None
+        return PerChannel(dtype, axis % tensor.dim())
+
+    def prepare(logical_path: str, tensor: torch.Tensor, tracing: bool) -> torch.Tensor:
+        spec = applies(logical_path, tensor)
+        if spec is None:
+            return tensor
+        if tracing:
+            return _Traced(tensor.shape, dtype)
+        scales, zps = per_channel_qparams(tensor, dtype, spec.axis)
+        x = tensor.detach().float()
+        return torch.quantize_per_channel(x, scales.to(x.device), zps.to(x.device), spec.axis, dtype)
+
+    prepare.tsnap_quant = applies  # type: ignore[attr-defined]
+    return prepare
+
+
 def fused_quant_of(func, tensor: torch.Tensor):
-    """(qdtype, scale, zero_point) when ``func`` is a recognised quantise-on-save hook for ``tensor``, else None."""
+    """(qdtype, scale, zero_point) when ``func`` is a recognised per-tensor quantise-on-save hook for ``tensor``, a
+    ``PerChannel`` when it is a per-channel one, else None."""
     args = []
     inner = func
     while isinstance(inner, functools.partial):

@@ -331,12 +331,7 @@ def _read_once_eligible(pg: Optional[PGWrapper]) -> bool:
 
 
 def _shift_descs(descs, delta: int):
-    out = []
-    for d in descs:
-        c = _native.CopyDesc.from_buffer_copy(d)
-        c.src_addr = d.src_addr + delta
-        out.append(c)
-    return out
+    return [_native.rebase(d, delta) for d in descs]
 
 
 def _execute_shared_reads(pg: PGWrapper, root: str, shared: List[Tuple[Tuple[str, int, int], list, list]], owner: Dict[Tuple[str, int, int], int]) -> int:
@@ -431,7 +426,7 @@ async def execute_read_reqs(
     candidates: List[Tuple[Tuple[str, int, int], list, list]] = []
     described_reqs = []
     for rr in read_reqs:
-        described = describe_consumer(rr.buffer_consumer) if root is not None else None
+        described = describe_consumer(rr.buffer_consumer, root) if root is not None else None
         if described is not None and not _one_device(described[1]):
             described = None
         if described is not None:
