@@ -201,20 +201,21 @@ def test_quantize_on_save_matches_torch_and_the_reference_format(tmp_path):
             assert (tgt[k] - st[k]).abs().max().item() <= scale * 0.5 + 1e-6, k
 
 
-@pytest.mark.parametrize("batching", [True, False])
-def test_async_take_counts_cpu_copies_against_the_memory_budget(tmp_path, monkeypatch, batching):
+@pytest.mark.parametrize("batching,quantize", [(True, False), (False, False), (True, True)], ids=["True", "False", "quantize_on_save"])
+def test_async_take_counts_cpu_copies_against_the_memory_budget(tmp_path, monkeypatch, batching, quantize):
     """async_take may hand control back while the engine still reads host memory, so CPU tensors get a private copy —
     but only while the per-rank memory budget lasts (the reference gates staging on it, T:scheduler.py:259-281);
     what does not fit is written out before async_take returns, from the caller's memory.  Either way the snapshot
-    holds the values at the time of the call."""
+    holds the values at the time of the call.  Sources the pack kernel quantises are charged like any other."""
     import torchsnapshot_b200 as B
     from torchsnapshot_b200 import scheduler as S
 
     monkeypatch.setenv("TORCHSNAPSHOT_PER_RANK_MEMORY_BUDGET_BYTES", str(3 << 20))
     monkeypatch.setenv("TORCHSNAPSHOT_DISABLE_BATCHING", "0" if batching else "1")
     tensors = {f"t{i}": torch.full((1 << 18,), float(i)) for i in range(8)}  # 8 x 1 MiB
-    expect = {k: v.clone() for k, v in tensors.items()}
-    pending = B.Snapshot.async_take(str(tmp_path / "s"), {"m": B.StateDict(**tensors)})
+    hook = B.quantize_on_save(torch.qint8) if quantize else None
+    expect = {k: hook(f"m/{k}", v, False).dequantize() if quantize else v.clone() for k, v in tensors.items()}
+    pending = B.Snapshot.async_take(str(tmp_path / "s"), {"m": B.StateDict(**tensors)}, _custom_tensor_prepare_func=hook)
     cloned, in_place = S.LAST_STATS["host_clone_bytes"], S.LAST_STATS["host_blocking_bytes"]
     for v in tensors.values():
         v.add_(100.0)  # the caller owns its memory again
@@ -226,7 +227,7 @@ def test_async_take_counts_cpu_copies_against_the_memory_budget(tmp_path, monkey
         assert torch.equal(out[k], v), k
     # with room for everything nothing blocks
     monkeypatch.setenv("TORCHSNAPSHOT_PER_RANK_MEMORY_BUDGET_BYTES", str(64 << 20))
-    B.Snapshot.async_take(str(tmp_path / "s2"), {"m": B.StateDict(**tensors)}).wait()
+    B.Snapshot.async_take(str(tmp_path / "s2"), {"m": B.StateDict(**tensors)}, _custom_tensor_prepare_func=hook).wait()
     assert S.LAST_STATS["host_blocking_bytes"] == 0 and S.LAST_STATS["host_clone_bytes"] == 8 << 20
 
 

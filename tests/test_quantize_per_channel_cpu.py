@@ -12,9 +12,11 @@ import torch.multiprocessing as mp
 
 import torchsnapshot_b200 as B
 from torchsnapshot_b200 import _native
+from torchsnapshot_b200 import storage_plugin as SP
 from torchsnapshot_b200.io_preparers.tensor import TensorBufferConsumer
 from torchsnapshot_b200.prepare import per_channel_qparams
 from torchsnapshot_b200.serialization import per_channel_qtensor_from_bytes
+from torchsnapshot_b200.storage_plugins.fs import FSStoragePlugin
 from tests.util import HAVE_REF, REF_PARENT
 
 FLOATS = [torch.float32, torch.bfloat16, torch.float16, torch.float64]
@@ -60,6 +62,20 @@ def file_of(snap, root, key):
     return e, open(os.path.join(root, e.location), "rb").read()
 
 
+class Audited(FSStoragePlugin):
+    """Overrides write / read, so the engine leaves the I/O to it: the stage / consume seam does the rest."""
+
+    async def write(self, write_io):
+        return await super().write(write_io)
+
+    async def read(self, read_io):
+        return await super().read(read_io)
+
+
+def _no_codec(*a, **k):
+    raise AssertionError("per-channel restore fell back to the Python codec")
+
+
 @pytest.mark.parametrize("qdtype", [torch.qint8, torch.quint8])
 @pytest.mark.parametrize("dtype", FLOATS)
 @pytest.mark.parametrize("axis", [0, 1, -1])
@@ -80,10 +96,7 @@ def test_file_bytes_and_native_restore(qdtype, dtype, axis, tmp_path, monkeypatc
     assert e.serializer == "buffer_protocol" and raw == src["bias"].contiguous().view(torch.uint8).numpy().tobytes()
 
     # restore runs through the engine, not the Python codec
-    def no_codec(*a, **k):
-        raise AssertionError("per-channel restore fell back to the Python codec")
-
-    monkeypatch.setattr(TensorBufferConsumer, "deserialize_tensor", staticmethod(no_codec))
+    monkeypatch.setattr(TensorBufferConsumer, "deserialize_tensor", staticmethod(_no_codec))
     tgt = {k: torch.full_like(v, 123.0) for k, v in src.items()}
     B.Snapshot(root).restore({"m": B.StateDict(**tgt)})
     for key in ("w", "w_t", "narrow", "cube"):
@@ -190,16 +203,6 @@ def test_async_take_copies_cpu_sources(tmp_path):
 
 
 def test_plugin_that_overrides_io_gets_the_same_bytes(tmp_path, monkeypatch):
-    from torchsnapshot_b200 import storage_plugin as SP
-    from torchsnapshot_b200.storage_plugins.fs import FSStoragePlugin
-
-    class Audited(FSStoragePlugin):  # overrides write / read: the stage / consume seam does the rest
-        async def write(self, write_io):
-            return await super().write(write_io)
-
-        async def read(self, read_io):
-            return await super().read(read_io)
-
     monkeypatch.setattr(SP, "FSStoragePlugin", Audited)
     src = sources(torch.float32)
     root = str(tmp_path / "s")
@@ -268,6 +271,16 @@ def test_bad_scheme_and_missing_record_are_rejected():
 
 
 def test_corrupt_header_and_size_give_clear_errors(tmp_path):
+    _corrupt_header_and_size(tmp_path)
+
+
+def test_corrupt_header_and_size_give_clear_errors_through_an_io_plugin(tmp_path, monkeypatch):
+    """The stage / consume seam reads the layout from the buffer it is handed and fails the same way."""
+    monkeypatch.setattr(SP, "FSStoragePlugin", Audited)
+    _corrupt_header_and_size(tmp_path)
+
+
+def _corrupt_header_and_size(tmp_path):
     x = torch.randn(10, 12)
     root = str(tmp_path / "s")
     snap = take(root, {"w": x}, B.quantize_on_save(torch.qint8, axis=0))
@@ -291,9 +304,11 @@ def _full():
     return torch.randn(ROWS, COLS, generator=torch.Generator().manual_seed(3)) * torch.linspace(0.5, 4, COLS)
 
 
-def _worker(rank, world, store_path, root):
+def _worker(rank, world, store_path, root, audited):
     from torch.distributed._shard.sharded_tensor import Shard, ShardedTensor, ShardMetadata
 
+    if audited:
+        SP.FSStoragePlugin = Audited  # a process of its own
     dist.init_process_group("gloo", init_method=f"file://{store_path}", rank=rank, world_size=world)
     full, step = _full(), ROWS // world
     local = full[rank * step : (rank + 1) * step].contiguous()
@@ -302,7 +317,8 @@ def _worker(rank, world, store_path, root):
     )
     B.Snapshot.take(os.path.join(root, "snap"), {"m": B.StateDict(t=st)}, _custom_tensor_prepare_func=B.quantize_on_save(torch.qint8, axis=1))
     dist.barrier()
-    # resharded restore: every rank reads a column band that crosses both saved pieces
+    # resharded restore: every rank reads a column band that crosses both saved pieces, and the engine dequantises it
+    TensorBufferConsumer.deserialize_tensor = staticmethod(_no_codec)
     cols = COLS // world
     band = torch.zeros(ROWS, cols)
     tgt = ShardedTensor._init_from_local_shards(
@@ -316,9 +332,18 @@ def _worker(rank, world, store_path, root):
 
 
 def test_two_rank_resharded_restore(tmp_path):
+    _two_rank_resharded_restore(tmp_path, audited=False)
+
+
+def test_two_rank_resharded_restore_through_an_io_plugin(tmp_path):
+    """The stage / consume seam dequantises reshard overlaps on the engine as well."""
+    _two_rank_resharded_restore(tmp_path, audited=True)
+
+
+def _two_rank_resharded_restore(tmp_path, audited):
     store = tempfile.NamedTemporaryFile(delete=False)
     try:
-        mp.spawn(_worker, args=(2, store.name, str(tmp_path)), nprocs=2, join=True)
+        mp.spawn(_worker, args=(2, store.name, str(tmp_path), audited), nprocs=2, join=True)
     finally:
         if os.path.exists(store.name):
             os.unlink(store.name)

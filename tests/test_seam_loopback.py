@@ -54,6 +54,18 @@ def test_tensor_round_trip_every_dtype(dtype):
             assert store["0/x"] == wire_bytes(view)
 
 
+def test_hook_whose_output_differs_from_its_trace_fails_to_stage():
+    """The entry was planned from the traced dtype; writing the processed tensor's bytes would not match it."""
+
+    def widens_late(t, tracing):
+        return t if tracing else t.double()
+
+    entry, wrs = TensorIOPreparer.prepare_write("0/x", torch.ones(4, 3), _tensor_prepare_func=widens_late)
+    assert entry.serializer == "buffer_protocol" and entry.dtype == "torch.float32"
+    with pytest.raises(RuntimeError, match="0/x"):
+        fulfil([], wrs)
+
+
 @pytest.mark.parametrize("limit", [1, 97, 1000, 10**6])
 def test_tiled_read_strided_offset_prime_targets(limit):
     # reference tests/test_tensor_io_preparer.py:159-183

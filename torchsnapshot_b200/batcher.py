@@ -19,13 +19,11 @@ from collections import defaultdict
 from concurrent.futures import Executor
 from typing import Dict, List, Optional, Tuple
 
-import torch
-
-from . import _native
 from .io_preparers.tensor import TensorBufferStager, current_stream_of, engine_for
 from .io_types import BufferConsumer, BufferStager, BufferType, ReadReq, WriteReq
 from .knobs import get_slab_size_threshold_bytes
 from .manifest import ChunkedTensorEntry, DTensorEntry, Entry, ShardedTensorEntry, TensorEntry
+from .native_plan import describe_stager
 from .serialization import Serializer
 
 ByteRange = Tuple[int, int]
@@ -51,24 +49,14 @@ class BatchedBufferStager(BufferStager):
         self.byte_range_to_buffer_stager = byte_range_to_buffer_stager
         self.slab_sz_bytes: int = end
 
-    def wire_nbytes(self) -> int:
-        return self.slab_sz_bytes
-
     def is_raw(self) -> bool:
         return all(isinstance(s, TensorBufferStager) and s.is_raw() for s in self.byte_range_to_buffer_stager.values())
 
-    def native_descs(self, wire_offset: int) -> Tuple[List["_native.CopyDesc"], List[torch.Tensor]]:
-        descs, keep = [], []
-        for (lo, hi), stager in self.byte_range_to_buffer_stager.items():
-            if stager.wire_nbytes() != hi - lo:
-                raise AssertionError(f"slab member size {stager.wire_nbytes()} does not match its byte range {(lo, hi)}")
-            d, k = stager.native_descs(wire_offset + lo)
-            descs += d
-            keep += k
-        return descs, keep
-
     async def stage_buffer(self, executor: Optional[Executor] = None) -> BufferType:
-        descs, keep = self.native_descs(0)
+        described = describe_stager(self)
+        if described is None:
+            raise AssertionError("a slab member is not a raw tensor that fills its byte range")
+        descs, keep, _ = described
         if not descs:
             return memoryview(bytes(self.slab_sz_bytes))
         if len({(t.device.type, t.device.index) for t in keep if t.is_cuda}) > 1:
@@ -176,14 +164,6 @@ class BatchedBufferConsumer(BufferConsumer):
 
     def is_raw(self) -> bool:
         return all(getattr(c, "is_raw", lambda: False)() for c in self.byte_range_to_buffer_consumer.values())
-
-    def native_descs(self, wire_offset: int) -> Tuple[List["_native.CopyDesc"], List[torch.Tensor]]:
-        descs, keep = [], []
-        for (lo, _hi), consumer in self.byte_range_to_buffer_consumer.items():
-            d, k = consumer.native_descs(wire_offset + lo)
-            descs += d
-            keep += k
-        return descs, keep
 
     async def consume_buffer(self, buf: bytes, executor: Optional[Executor] = None) -> None:
         view = memoryview(buf)

@@ -22,18 +22,9 @@ from .. import _native
 from ..io_types import BufferConsumer, Future, ReadReq, WriteReq
 from ..knobs import get_max_shard_size_bytes
 from ..manifest import Shard, ShardedTensorEntry, TensorEntry
-from ..serialization import string_to_dtype
-from .tensor import (
-    PICKLED,
-    RAW,
-    PrepareFunc,
-    TensorBufferConsumer,
-    TensorIOPreparer,
-    _raw_castable,
-    engine_for,
-    entry_nbytes,
-    tensor_copy,
-)
+from ..native_plan import RAW, describe_consumer, entry_nbytes, raw_castable
+from ..serialization import dtype_to_element_size, string_to_dtype
+from .tensor import PICKLED, PrepareFunc, TensorBufferConsumer, TensorIOPreparer, engine_for, tensor_copy
 
 Box = Tuple[List[int], List[int]]  # (offsets, sizes) in global coordinates
 
@@ -86,37 +77,14 @@ class ShardedTensorBufferConsumer(BufferConsumer):
         if self.entry.serializer != RAW:
             return False
         src = string_to_dtype(self.entry.dtype)
-        return all(_raw_castable(src, r.dst_tensor.dtype) for r in self.overlapping_regions)
-
-    def wire_nbytes(self) -> int:
-        return entry_nbytes(self.entry)
-
-    def native_descs(self, wire_offset: int) -> Tuple[List["_native.CopyDesc"], List[torch.Tensor]]:
-        shape = list(self.entry.shape)
-        dtype = string_to_dtype(self.entry.dtype)
-        esz = torch.empty(0, dtype=dtype).element_size()
-        strides = [1] * len(shape)
-        for i in range(len(shape) - 2, -1, -1):
-            strides[i] = strides[i + 1] * shape[i + 1]
-        descs, keep = [], []
-        for region in self.overlapping_regions:
-            dst = region.dst_tensor.detach()
-            first = 0
-            for dim, so, do, n in region.overlap_region:
-                dst = dst.narrow(dim, do, n)
-                first += so * strides[dim]
-            if dst.numel() == 0:
-                continue
-            descs.append(_native.load_desc(dst, wire_offset + first * esz - self.wire_skip, wire_dtype=dtype, wire_strides=strides))
-            keep.append(region.dst_tensor)
-        return descs, keep
+        return all(raw_castable(src, r.dst_tensor.dtype) for r in self.overlapping_regions)
 
     async def consume_buffer(self, buf: bytes, executor: Optional[Executor] = None) -> None:
         def work() -> None:
-            if self.is_raw():
-                descs, _ = self.native_descs(0)
-                if descs:
-                    engine_for(self.overlapping_regions[0].dst_tensor).consume(buf, descs)
+            described = describe_consumer(self, buf=buf)
+            if described is not None:
+                if described[0]:
+                    engine_for(self.overlapping_regions[0].dst_tensor).consume(buf, described[0])
                 return
             if self.wire_skip or self.wire_len is not None:
                 raise AssertionError("partial reads are only planned for raw entries")
@@ -143,10 +111,8 @@ def needed_hull(entry: TensorEntry, regions: List[_OverlappingRegion]) -> Option
     if entry.serializer != RAW:
         return None
     shape = list(entry.shape)
-    esz = torch.empty(0, dtype=string_to_dtype(entry.dtype)).element_size()
-    strides = [1] * len(shape)
-    for i in range(len(shape) - 2, -1, -1):
-        strides[i] = strides[i + 1] * shape[i + 1]
+    esz = dtype_to_element_size(string_to_dtype(entry.dtype))
+    strides = _native._c_strides(shape)
     lo, hi = None, None
     for r in regions:
         first = sum(so * strides[d] for d, so, _, _ in r.overlap_region)

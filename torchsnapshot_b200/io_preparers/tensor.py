@@ -4,15 +4,14 @@ Reference behaviour being replaced (T:io_preparers/tensor.py):
   * prepare_write (50-89)   -> TensorEntry + one WriteReq whose stager owns the (view of the) tensor
   * stage_buffer (240-271)  -> pageable ``tensor.to("cpu")`` in a thread, then a memoryview
   * consume_buffer (331-340)-> frombuffer + ``dst.copy_(src)`` (pageable H2D)
-Here the stager/consumer only *describe* the copy (``native_descs``); the engine executes all of them
-together: one pack/scatter kernel launch, pinned ring, native file I/O.  The asyncio methods remain
-for storage plugins the engine cannot drive directly and run the same kernels through the stage /
+Here ``native_plan.describe_stager`` / ``describe_consumer`` turn the stager/consumer into copy descriptors; the
+engine executes all of them together: one pack/scatter kernel launch, pinned ring, native file I/O.  The asyncio
+methods remain for storage plugins the engine cannot drive directly and run the same descriptors through the stage /
 consume seam of the C ABI."""
 from __future__ import annotations
 
 import asyncio
 import math
-import struct
 from concurrent.futures import Executor
 from typing import Any, Callable, List, Optional, Tuple, Union
 
@@ -21,42 +20,24 @@ import torch
 from .. import _native
 from ..io_types import BufferConsumer, BufferStager, BufferType, Future, ReadReq, WriteReq
 from ..manifest import ChunkedTensorEntry, TensorEntry
+from ..native_plan import RAW, describe_consumer, describe_stager, entry_nbytes, raw_castable
+from ..prepare import _FLOATS, PER_CHANNEL_QTENSOR, PER_TENSOR_QTENSOR, PerChannel, fused_quant_of
 from ..serialization import (
     BUFFER_PROTOCOL_SUPPORTED_DTYPES,
     SUPPORTED_QUANTIZED_DTYPES,
     Serializer,
     dtype_to_element_size,
     dtype_to_string,
+    per_channel_qtensor_from_bytes,
+    per_tensor_qtensor_from_bytes,
     string_to_dtype,
     tensor_from_memoryview,
     torch_load_from_bytes,
     torch_save_as_bytes,
 )
 
-RAW = Serializer.BUFFER_PROTOCOL.value
 PICKLED = Serializer.TORCH_SAVE.value
-from ..prepare import PER_CHANNEL_QTENSOR, PER_TENSOR_QTENSOR, PerChannel, fused_quant_of  # noqa: E402
-from ..serialization import per_channel_qtensor_from_bytes, per_tensor_qtensor_from_bytes  # noqa: E402
 PrepareFunc = Callable[[torch.Tensor, bool], torch.Tensor]
-
-
-def entry_nbytes(entry: TensorEntry) -> int:
-    n = dtype_to_element_size(string_to_dtype(entry.dtype))
-    for s in entry.shape:
-        n *= s
-    if entry.serializer == PER_TENSOR_QTENSOR:
-        n += 16  # [q_scale: double][q_zero_point: int64] behind the int_repr bytes (T:serialization.py:278-310)
-    elif entry.serializer == PER_CHANNEL_QTENSOR:
-        n += 8  # the axis header; the 16 B per channel behind the body depend on the axis, which only the file records
-    return n
-
-
-def per_channel_wire_nbytes(shape, axis: int) -> int:
-    """Size of a per-channel file: [axis][int_repr bytes][scales: f64 x C][zero_points: i64 x C]."""
-    numel = 1
-    for s in shape:
-        numel *= s
-    return 8 + numel + 16 * shape[axis]
 
 
 def engine_for(t: torch.Tensor) -> "_native.Engine":
@@ -99,45 +80,22 @@ class TensorBufferStager(BufferStager):
             t = self._tensor_prepare_func(t, False).detach()
         return t
 
-    def wire_nbytes(self) -> int:
-        if isinstance(self.qparams, PerChannel):
-            return per_channel_wire_nbytes(list(self.entry.shape), self.qparams.axis)
-        return entry_nbytes(self.entry)
-
-    def native_descs(self, wire_offset: int) -> Tuple[List["_native.CopyDesc"], List[torch.Tensor]]:
-        if self.qparams is not None:
-            t = self.tensor.detach()
-            if self.is_async_snapshot and t.device.type == "cpu":
-                t = t.clone()
-            if isinstance(self.qparams, PerChannel):
-                if _native.needs_contiguous_copy(t):
-                    t = t.contiguous()
-                d = _native.save_desc(t, wire_offset + 8, wire_dtype=self.qparams.dtype, axis=self.qparams.axis)
-                return [d], [t]
-            qdtype, scale, zp = self.qparams
-            return [_native.save_desc(t, wire_offset, wire_dtype=qdtype, qparams=(scale, zp))], [t]
-        t = self.source()
-        if t.numel() == 0:
-            return [], []
-        if _native.needs_contiguous_copy(t):
-            t = t.contiguous()
-        elif self.is_async_snapshot and t.device.type == "cpu":
-            # host memory is read while the snapshot drains in the background: take a private copy so
-            # that later in-place updates (e.g. Adam's CPU `step` counters) cannot leak into it
-            t = t.clone()
-        return [_native.save_desc(t, wire_offset)], [t]
-
     # ---- asyncio seam ---------------------------------------------------------------------------
     async def stage_buffer(self, executor: Optional[Executor] = None) -> BufferType:
-        if not self.is_raw() and self.qparams is None:
+        described = describe_stager(self)
+        if described is None:
+            if self.is_raw():
+                raise RuntimeError(
+                    f"{self.entry.location}: the prepare func's output does not match the entry it traced "
+                    f"({self.entry.dtype}, shape {list(self.entry.shape)})"
+                )
             # complex / quantized tensors: unchanged torch.save path (out of scope of the engine)
             t = self.source()
             cpu = t.cpu() if t.device.type != "cpu" else t
             if cpu.numel() != cpu.untyped_storage().nbytes() // max(cpu.element_size(), 1):
                 cpu = cpu.clone()
             return torch_save_as_bytes(cpu)
-        descs, keep = self.native_descs(0)
-        nbytes = self.wire_nbytes()
+        descs, keep, nbytes = described
         if not descs:
             return memoryview(b"")
         t = keep[0]
@@ -157,19 +115,7 @@ class TensorBufferConsumer(BufferConsumer):
         self.entry = entry
 
     def is_raw(self) -> bool:
-        return self.entry.serializer == RAW and _raw_castable(string_to_dtype(self.entry.dtype), self.tensor.dtype)
-
-    def wire_nbytes(self) -> int:
-        return entry_nbytes(self.entry)
-
-    def native_descs(self, wire_offset: int) -> Tuple[List["_native.CopyDesc"], List[torch.Tensor]]:
-        """The destination receives the whole saved tensor (dtype-converting when they differ)."""
-        dst = self.tensor.detach()
-        if dst.numel() == 0:
-            return [], []
-        if list(dst.shape) != list(self.entry.shape):
-            raise RuntimeError(f"shape mismatch: saved {self.entry.shape}, destination {list(dst.shape)}")
-        return [_native.load_desc(dst, wire_offset, wire_dtype=string_to_dtype(self.entry.dtype))], [dst]
+        return self.entry.serializer == RAW and raw_castable(string_to_dtype(self.entry.dtype), self.tensor.dtype)
 
     @staticmethod
     def deserialize_tensor(buf: bytes, entry: TensorEntry) -> torch.Tensor:
@@ -183,28 +129,13 @@ class TensorBufferConsumer(BufferConsumer):
             return per_channel_qtensor_from_bytes(bytes(buf), string_to_dtype(entry.dtype), list(entry.shape))
         raise ValueError(f"Unrecognized serializer: {entry.serializer}.")
 
-    def per_channel_descs(self, buf) -> Optional[List["_native.CopyDesc"]]:
-        """Dequantising scatter of a per-channel image in ``buf`` into a float target, or None for other entries."""
-        shape = list(self.entry.shape)
-        if self.entry.serializer != PER_CHANNEL_QTENSOR or self.tensor.dtype not in _FLOATS or list(self.tensor.shape) != shape:
-            return None
-        axis = struct.unpack_from("<q", buf, 0)[0] if len(buf) >= 8 else -1
-        if not 0 <= axis < len(shape) or len(buf) != per_channel_wire_nbytes(shape, axis):
-            raise RuntimeError(f"per-channel image of {len(buf)} bytes with axis {axis} does not fit shape {shape}")
-        if self.tensor.numel() == 0:
-            return []
-        qdtype = string_to_dtype(self.entry.dtype)
-        return [_native.per_channel(_native.load_desc(self.tensor.detach(), 8, wire_dtype=qdtype), shape, axis, 8)]
-
     async def consume_buffer(self, buf: bytes, executor: Optional[Executor] = None) -> None:
         def work() -> None:
-            quantised = self.per_channel_descs(buf)
-            if self.is_raw() or quantised is not None:
-                descs = quantised if quantised is not None else self.native_descs(0)[0]
-                if descs:
-                    engine_for(self.tensor).consume(buf, descs)
-            else:
+            described = describe_consumer(self, buf=buf)
+            if described is None:
                 tensor_copy(self.tensor, self.deserialize_tensor(buf, self.entry))
+            elif described[0]:
+                engine_for(self.tensor).consume(buf, described[0])
 
         if executor is not None:
             await asyncio.get_running_loop().run_in_executor(executor, work)
@@ -228,16 +159,6 @@ class _DecodingConsumer(BufferConsumer):
 
     def get_consuming_cost_bytes(self) -> int:
         return 2 * entry_nbytes(self.entry)
-
-
-_FLOATS = (torch.float16, torch.bfloat16, torch.float32, torch.float64)
-
-
-def _raw_castable(src: torch.dtype, dst: torch.dtype) -> bool:
-    """dtype pairs the scatter kernel handles itself; others fall back to Tensor.copy_ semantics."""
-    if src == dst:
-        return src in BUFFER_PROTOCOL_SUPPORTED_DTYPES
-    return src in _FLOATS and dst in _FLOATS
 
 
 def tensor_copy(dst: torch.Tensor, src: torch.Tensor) -> None:

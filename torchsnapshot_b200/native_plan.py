@@ -1,10 +1,11 @@
-"""Turns stagers / consumers into C-ABI copy descriptors.
+"""Turns stagers / consumers into C-ABI copy descriptors: the only code that knows how a tensor maps to its wire image.
 
-Works on this package's classes and, by duck typing on the attribute names they share, on the
-reference's own ``TensorBufferStager`` / ``BatchedBufferStager`` / ``GPUBatchedBufferStager`` /
-``TensorBufferConsumer`` / ``ShardedTensorBufferConsumer`` / ``BatchedBufferConsumer`` objects
-(T:io_preparers/tensor.py:223-350, T:batcher.py:51-162,358-384, T:io_preparers/sharded_tensor.py:285-323) —
-which is what lets ``torchsnapshot_b200.install()`` put the engine underneath an unmodified torchsnapshot."""
+Both the engine's file jobs (``scheduler``) and the asyncio ``stage_buffer`` / ``consume_buffer`` seam use it.  It works
+on this package's classes and, by duck typing on the attribute names they share, on the reference's own
+``TensorBufferStager`` / ``BatchedBufferStager`` / ``GPUBatchedBufferStager`` / ``TensorBufferConsumer`` /
+``ShardedTensorBufferConsumer`` / ``BatchedBufferConsumer`` objects (T:io_preparers/tensor.py:223-350,
+T:batcher.py:51-162,358-384, T:io_preparers/sharded_tensor.py:285-323) — which is what lets
+``torchsnapshot_b200.install()`` put the engine underneath an unmodified torchsnapshot."""
 from __future__ import annotations
 
 import os
@@ -14,25 +15,34 @@ from typing import Any, List, Optional, Tuple
 import torch
 
 from . import _native
-from .prepare import PER_CHANNEL_QTENSOR
-from .serialization import BUFFER_PROTOCOL_SUPPORTED_DTYPES
+from .prepare import _FLOATS, PER_CHANNEL_QTENSOR, PER_TENSOR_QTENSOR, PerChannel, fused_cast_of
+from .serialization import BUFFER_PROTOCOL_SUPPORTED_DTYPES, Serializer, dtype_to_element_size, string_to_dtype
 
-RAW = "buffer_protocol"
-_FLOATS = (torch.float16, torch.bfloat16, torch.float32, torch.float64)
+RAW = Serializer.BUFFER_PROTOCOL.value
 _DTYPES = {str(dt): dt for dt in BUFFER_PROTOCOL_SUPPORTED_DTYPES}
 
 Described = Tuple[List["_native.CopyDesc"], List[torch.Tensor], int]  # descriptors, keep-alive, wire bytes
 
 
-def _entry_nbytes(entry: Any) -> int:
-    n = torch.empty(0, dtype=_DTYPES[entry.dtype]).element_size()
+def entry_nbytes(entry: Any, axis: Optional[int] = None) -> int:
+    """Payload size of a tensor entry.  A per-tensor quantised one carries ``[q_scale: double][q_zero_point: int64]``
+    behind the int_repr bytes (T:serialization.py:278-310); a per-channel one ``[axis: int64]`` before them and, given
+    the axis (only the file records it), ``[scales: f64 x C][zero_points: i64 x C]`` behind them."""
+    n = dtype_to_element_size(string_to_dtype(entry.dtype))
     for s in entry.shape:
         n *= s
+    if entry.serializer == PER_TENSOR_QTENSOR:
+        n += 16
+    elif entry.serializer == PER_CHANNEL_QTENSOR:
+        n += 8 + (16 * entry.shape[axis] if axis is not None else 0)
     return n
 
 
-def _castable(src: torch.dtype, dst: torch.dtype) -> bool:
-    return src == dst or (src in _FLOATS and dst in _FLOATS)
+def raw_castable(src: torch.dtype, dst: torch.dtype) -> bool:
+    """dtype pairs the scatter kernel handles itself; others fall back to Tensor.copy_ semantics."""
+    if src == dst:
+        return src in BUFFER_PROTOCOL_SUPPORTED_DTYPES
+    return src in _FLOATS and dst in _FLOATS
 
 
 # ---- save side -----------------------------------------------------------------------------------
@@ -64,45 +74,49 @@ class HostCloneBudget:
         return b
 
 
-def _describe_tensor_stager(st: Any, offset: int, clones: Optional[HostCloneBudget] = None) -> Optional[Described]:
+def _describe_tensor_stager(st: Any, offset: int, clones: Optional[HostCloneBudget]) -> Optional[Described]:
     entry = getattr(st, "entry", None)
     tensor = getattr(st, "tensor", None)
-    if entry is not None and isinstance(tensor, torch.Tensor) and getattr(st, "qparams", None) is not None:
-        # quantise-on-save: the pack kernel produces int_repr + trailer, or the engine the whole per-channel image
-        # (prepare.quantize_on_save)
-        descs, keep = st.native_descs(offset)
-        return descs, keep, st.wire_nbytes()
-    if entry is None or not isinstance(tensor, torch.Tensor) or getattr(entry, "serializer", None) != RAW:
-        return None
-    if entry.dtype not in _DTYPES:
+    serializer = getattr(entry, "serializer", None)
+    if not isinstance(tensor, torch.Tensor):
         return None
     t = tensor.detach()
-    func = getattr(st, "_tensor_prepare_func", None)
-    wire_dtype = None
-    if func is not None:
-        from .prepare import fused_cast_of
-
-        wire_dtype = fused_cast_of(func, t)
-        if wire_dtype is None:
-            t = func(t, False).detach()  # persist the processed tensor (DESIGN.md §6)
-        # else: a pure float cast — the pack kernel converts while it gathers, no processed tensor is materialised
-    if str(wire_dtype or t.dtype) != entry.dtype or list(t.shape) != list(entry.shape):
+    # quantise-on-save (prepare.quantize_on_save): the stager computed the parameters once, when it was created
+    q = getattr(st, "qparams", None) if serializer in (PER_TENSOR_QTENSOR, PER_CHANNEL_QTENSOR) else None
+    wire_dtype = qparams = axis = None
+    if isinstance(q, PerChannel):
+        # the engine writes the axis header, the int body behind it and the channel parameters behind the body
+        wire_dtype, axis, nbytes, offset = q.dtype, q.axis, entry_nbytes(entry, q.axis), offset + 8
+    elif q is not None:
+        # the pack kernel writes int_repr + the 16-byte trailer
+        wire_dtype, qparams, nbytes = q[0], q[1:], entry_nbytes(entry)
+    elif serializer == RAW and entry.dtype in _DTYPES:
+        func = getattr(st, "_tensor_prepare_func", None)
+        if func is not None:
+            wire_dtype = fused_cast_of(func, t)
+            if wire_dtype is None:
+                t = func(t, False).detach()  # persist the processed tensor (DESIGN.md §6)
+            # else: a pure float cast — the pack kernel converts while it gathers, no processed tensor is materialised
+        if str(wire_dtype or t.dtype) != entry.dtype or list(t.shape) != list(entry.shape):
+            return None
+        nbytes = entry_nbytes(entry)
+        if t.numel() == 0:
+            return [], [], nbytes
+    else:
         return None
-    nbytes = _entry_nbytes(entry)
-    if t.numel() == 0:
-        return [], [], nbytes
     if _native.needs_contiguous_copy(t):
         t = t.contiguous()
     elif getattr(st, "is_async_snapshot", False) and t.device.type == "cpu":
         # host memory is read after async_take returned: a private copy while the budget lasts, else a blocking request
         if clones is None or clones.admit(t.numel() * t.element_size()):
             t = t.clone()
-    return [_native.save_desc(t, offset, wire_dtype=wire_dtype)], [t], nbytes
+    return [_native.save_desc(t, offset, wire_dtype=wire_dtype, qparams=qparams, axis=axis)], [t], nbytes
 
 
 def describe_stager(st: Any, clones: Optional[HostCloneBudget] = None) -> Optional[Described]:
     """(descriptors, keep-alive tensors, wire size) of one WriteReq's stager, or None when it has to go
-    through its own ``stage_buffer`` (pickled objects, complex / quantized tensors, foreign stagers)."""
+    through its own ``stage_buffer`` (pickled objects, complex / quantized tensors, foreign stagers).
+    Without ``clones`` every CPU source of an async snapshot is copied."""
     members = getattr(st, "byte_range_to_buffer_stager", None)
     if members is not None:
         descs: List[Any] = []
@@ -120,107 +134,76 @@ def describe_stager(st: Any, clones: Optional[HostCloneBudget] = None) -> Option
 
 
 # ---- restore side ----------------------------------------------------------------------------------
-def per_channel_layout(path: str, entry: Any) -> Tuple[int, int]:
-    """(file size, axis) of a per-channel file, from the file itself: the manifest records neither."""
-    from .io_preparers.tensor import per_channel_wire_nbytes
-
+def per_channel_axis(head: bytes, size: int, entry: Any, where: str) -> int:
+    """Axis of a per-channel image of ``size`` bytes that starts with the 8 bytes ``head``, checked against the entry's
+    shape: the manifest records neither the axis nor the size.  ``where`` names the image in the error."""
     shape = list(entry.shape)
-    size = os.stat(path).st_size
-    with open(path, "rb") as f:
-        head = f.read(8)
     axis = struct.unpack("<q", head)[0] if len(head) == 8 else -1
     if not 0 <= axis < len(shape):
-        raise RuntimeError(f"{path}: per-channel header names axis {axis}, but the saved tensor has shape {shape}")
-    if size != per_channel_wire_nbytes(shape, axis):
-        raise RuntimeError(f"{path}: {size} bytes, but a per-channel image of shape {shape} along axis {axis} has "
-                           f"{per_channel_wire_nbytes(shape, axis)}")
-    return size, axis
+        raise RuntimeError(f"{where}: per-channel header names axis {axis}, but the saved tensor has shape {shape}")
+    want = entry_nbytes(entry, axis)
+    if size != want:
+        raise RuntimeError(f"{where}: {size} bytes, but a per-channel image of shape {shape} along axis {axis} has {want}")
+    return axis
 
 
-def _describe_per_channel_consumer(c: Any, offset: int, root: Optional[str]) -> Optional[Described]:
-    """Dequantising scatter of a per-channel entry into float targets (the whole tensor or reshard overlaps)."""
-    entry = c.entry
-    regions = getattr(c, "overlapping_regions", None)
-    targets = [r.dst_tensor for r in regions] if regions is not None else [getattr(c, "tensor", None)]
-    if root is None or getattr(entry, "byte_range", None) is not None or int(getattr(c, "wire_skip", 0) or 0):
-        return None
-    if not all(isinstance(t, torch.Tensor) and t.dtype in _FLOATS for t in targets):
-        return None  # quantised targets keep torch's own copy semantics
-    nbytes, axis = per_channel_layout(os.path.join(root, entry.location), entry)
-    qdtype = {"torch.qint8": torch.qint8, "torch.quint8": torch.quint8}[entry.dtype]
-    shape = list(entry.shape)
-    strides = _native._c_strides(shape)
-    body = offset + 8
-
-    def desc(dst: torch.Tensor, first: int):
-        return _native.per_channel(_native.load_desc(dst, body + first, wire_dtype=qdtype, wire_strides=strides), shape, axis, body)
-
-    if regions is None:
-        dst = c.tensor.detach()
-        if list(dst.shape) != shape:
-            return None
-        return ([desc(dst, 0)] if dst.numel() else []), [dst], nbytes
-    descs, keep = [], []
-    for region in regions:
-        dst = region.dst_tensor.detach()
-        first = 0
-        for dim, so, do, n in region.overlap_region:
-            dst = dst.narrow(dim, do, n)
-            first += so * strides[dim]
-        if dst.numel():
-            descs.append(desc(dst, first))
-            keep.append(region.dst_tensor)
-    return descs, keep, nbytes
-
-
-def _describe_tensor_consumer(c: Any, offset: int, root: Optional[str] = None) -> Optional[Described]:
+def _describe_tensor_consumer(c: Any, offset: int, root: Optional[str] = None, buf: Any = None) -> Optional[Described]:
     entry = getattr(c, "entry", None)
-    if entry is not None and getattr(entry, "serializer", None) == PER_CHANNEL_QTENSOR:
-        return _describe_per_channel_consumer(c, offset, root)
-    if entry is None or getattr(entry, "serializer", None) != RAW or entry.dtype not in _DTYPES:
+    serializer = getattr(entry, "serializer", None)
+    raw = serializer == RAW and entry.dtype in _DTYPES
+    if not raw and serializer != PER_CHANNEL_QTENSOR:
         return None
-    src_dtype = _DTYPES[entry.dtype]
-    nbytes = _entry_nbytes(entry)
+    shape = list(entry.shape)
     regions = getattr(c, "overlapping_regions", None)
     if regions is not None:
         # reshard-on-load: each overlap is one strided copy out of the saved piece's C-order image
-        shape = list(entry.shape)
-        esz = torch.empty(0, dtype=src_dtype).element_size()
-        strides = [1] * len(shape)
-        for i in range(len(shape) - 2, -1, -1):
-            strides[i] = strides[i + 1] * shape[i + 1]
-        descs, keep = [], []
-        skip = int(getattr(c, "wire_skip", 0) or 0)
-        if getattr(c, "wire_len", None) is not None:
-            nbytes = int(c.wire_len)
-        for region in regions:
-            dst = region.dst_tensor.detach()
-            if not _castable(src_dtype, dst.dtype) or dst.is_quantized:
-                return None
-            first = 0
-            for dim, so, do, n in region.overlap_region:
-                dst = dst.narrow(dim, do, n)
-                first += so * strides[dim]
-            if dst.numel() == 0:
-                continue
-            descs.append(_native.load_desc(dst, offset + first * esz - skip, wire_dtype=src_dtype, wire_strides=strides))
-            keep.append(region.dst_tensor)
-        return descs, keep, nbytes
-    tensor = getattr(c, "tensor", None)
-    if not isinstance(tensor, torch.Tensor) or tensor.is_quantized or not _castable(src_dtype, tensor.dtype):
-        return None
-    dst = tensor.detach()
-    if list(dst.shape) != list(entry.shape):
-        return None
-    if dst.numel() == 0:
-        return [], [], nbytes
-    return [_native.load_desc(dst, offset, wire_dtype=src_dtype)], [dst], nbytes
+        targets = [(r.dst_tensor, r.overlap_region) for r in regions]
+    else:
+        tensor = getattr(c, "tensor", None)
+        if not isinstance(tensor, torch.Tensor) or list(tensor.shape) != shape:
+            return None
+        targets = [(tensor, ())]
+    skip = int(getattr(c, "wire_skip", 0) or 0)
+    axis = None
+    if raw:
+        wire_dtype = _DTYPES[entry.dtype]
+        if not all(raw_castable(wire_dtype, t.dtype) for t, _ in targets):
+            return None
+        nbytes = entry_nbytes(entry) if getattr(c, "wire_len", None) is None else int(c.wire_len)
+        esz, body = dtype_to_element_size(wire_dtype), offset - skip
+    else:
+        # dequantising scatter into float targets; quantised targets keep torch's own copy semantics
+        if skip or getattr(entry, "byte_range", None) is not None or (root is None and buf is None):
+            return None
+        if not all(t.dtype in _FLOATS for t, _ in targets):
+            return None
+        if buf is None:
+            where = os.path.join(root, entry.location)
+            nbytes = os.stat(where).st_size
+            with open(where, "rb") as f:
+                head = f.read(8)
+        else:
+            where, nbytes, head = entry.location, len(buf), bytes(buf[:8])
+        axis = per_channel_axis(head, nbytes, entry, where)
+        wire_dtype, esz, body = string_to_dtype(entry.dtype), 1, offset + 8
+    strides = _native._c_strides(shape)
+    descs, keep = [], []
+    for tensor, narrows in targets:
+        dst, first = tensor.detach(), 0
+        for dim, so, do, n in narrows:
+            dst = dst.narrow(dim, do, n)
+            first += so * strides[dim]
+        if dst.numel():
+            d = _native.load_desc(dst, body + first * esz, wire_dtype=wire_dtype, wire_strides=strides)
+            descs.append(d if axis is None else _native.per_channel(d, shape, axis, body))
+            keep.append(tensor)
+    return descs, keep, nbytes
 
 
-def describe_consumer(c: Any, root: Optional[str] = None) -> Optional[Described]:
+def describe_consumer(c: Any, root: Optional[str] = None, buf: Any = None) -> Optional[Described]:
     """(descriptors, keep-alive tensors, wire size) of one ReadReq's consumer, or None when it has to go through its own
-    ``consume_buffer``.  ``root``: directory the entries' locations are relative to; per-channel entries need it to read
-    their layout from the file."""
+    ``consume_buffer``.  A per-channel entry's layout is read from ``buf`` (the bytes the consumer was handed) or else
+    from its file under ``root``, the directory the entries' locations are relative to."""
     members = getattr(c, "byte_range_to_buffer_consumer", None)
     if members is not None:
         descs: List[Any] = []
@@ -232,7 +215,7 @@ def describe_consumer(c: Any, root: Optional[str] = None) -> Optional[Described]
             descs += one[0]
             keep += one[1]
         return descs, keep, int(getattr(c, "buf_sz_bytes", 0))
-    return _describe_tensor_consumer(c, 0, root)
+    return _describe_tensor_consumer(c, 0, root, buf)
 
 
 def native_root(storage: Any, op: str = "write") -> Optional[str]:
