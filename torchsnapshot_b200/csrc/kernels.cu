@@ -676,18 +676,32 @@ __device__ __forceinline__ uint8_t quantize_elem(float x, double scale, int64_t 
     return (uint8_t)(int8_t)q;
 }
 
-__device__ __forceinline__ void convert_store(char* p, uint32_t ddt, const char* sp, uint32_t sdt, bool aligned) {
-    // <=32-bit float sources convert through fp32 (exact widening), fp64 sources narrow directly:
-    // the same single rounding step torch's copy kernel performs.
+// the n bytes of an element; byte by byte when the source is not element aligned (a wire member behind an odd-sized
+// one in an unpadded slab)
+__device__ __forceinline__ uint64_t load_bits(const char* p, uint32_t n, bool aligned) {
+    if (aligned) return n == 8 ? *reinterpret_cast<const uint64_t*>(p) : n == 4 ? *reinterpret_cast<const uint32_t*>(p) : *reinterpret_cast<const uint16_t*>(p);
+    uint64_t v = 0;
+    for (int i = (int)n - 1; i >= 0; --i) v = (v << 8) | (uint8_t)p[i];
+    return v;
+}
+
+__device__ __forceinline__ void convert_store(char* p, uint32_t ddt, const char* sp, uint32_t sdt, bool src_aligned, bool aligned) {
+    // <=32-bit float sources convert through fp32 (exact widening, with no detour through double: that would quiet the
+    // signalling NaNs torch's bf16 -> fp32 widening keeps bit for bit).  fp64 sources narrow to fp32 and bf16 in one
+    // rounding step, and to fp16 through fp32: torch's copy kernel has no double -> half conversion (c10::Half is built
+    // from a float), so it rounds twice.
     if (sdt == TSNAP_F64) {
-        const double x = *reinterpret_cast<const double*>(sp);
+        const double x = __longlong_as_double((long long)load_bits(sp, 8, src_aligned));
         if (ddt == TSNAP_F32) { const float f = (float)x; store_bytes(p, &f, 4, aligned); }
-        else if (ddt == TSNAP_F16) { const __half h = __double2half(x); store_bytes(p, &h, 2, aligned); }
+        else if (ddt == TSNAP_F16) { const __half h = __float2half_rn((float)x); store_bytes(p, &h, 2, aligned); }
         else if (ddt == TSNAP_BF16) { const __nv_bfloat16 b = __float2bfloat16_rn((float)x); store_bytes(p, &b, 2, aligned); }
         else store_bytes(p, &x, 8, aligned);
         return;
     }
-    const float f = (float)load_elem(sp, sdt);
+    const uint32_t w = (uint32_t)load_bits(sp, sdt == TSNAP_F32 ? 4 : 2, src_aligned);
+    const float f = sdt == TSNAP_F32 ? __uint_as_float(w)
+                    : sdt == TSNAP_BF16 ? __bfloat162float(__ushort_as_bfloat16((unsigned short)w))
+                                        : __half2float(__ushort_as_half((unsigned short)w));
     if (ddt == TSNAP_F32) store_bytes(p, &f, 4, aligned);
     else if (ddt == TSNAP_F16) { const __half h = __float2half_rn(f); store_bytes(p, &h, 2, aligned); }
     else if (ddt == TSNAP_BF16) { const __nv_bfloat16 b = __float2bfloat16_rn(f); store_bytes(p, &b, 2, aligned); }
@@ -781,13 +795,16 @@ __device__ __noinline__ void tile_cast(const Member& m, uint32_t index) {
         }
         return;
     }
-    bool aligned = (m.dst % m.dst_esz) == 0;
-    for (uint32_t i = 0; i < m.nouter; ++i) aligned = aligned && ((uint64_t)m.dstride[i] % m.dst_esz) == 0;
+    bool aligned = (m.dst % m.dst_esz) == 0, src_aligned = (m.src % m.src_esz) == 0;
+    for (uint32_t i = 0; i < m.nouter; ++i) {
+        aligned = aligned && ((uint64_t)m.dstride[i] % m.dst_esz) == 0;
+        src_aligned = src_aligned && ((uint64_t)m.sstride[i] % m.src_esz) == 0;
+    }
     for (uint64_t e = e0 + threadIdx.x; e < e1; e += kLsuThreads) {
         const uint64_t row = e / m.inner, col = e - row * m.inner;
         int64_t so, dofs;
         outer_offsets(m, row, &so, &dofs);
-        convert_store(db + dofs + col * m.dst_esz, m.dst_dtype, sb + so + col * m.src_esz, m.src_dtype, aligned);
+        convert_store(db + dofs + col * m.dst_esz, m.dst_dtype, sb + so + col * m.src_esz, m.src_dtype, src_aligned, aligned);
     }
 }
 

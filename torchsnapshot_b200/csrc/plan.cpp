@@ -155,7 +155,6 @@ int normalize_copy(const tsnap_copy_desc& d, uint64_t wire_base, bool allow_bulk
         } else {
             m.inner = 1;
         }
-        if (m.src % es) return fail(TSNAP_EINVAL, "cast source is not element aligned");
     } else {
         if (nd > 0 && dims[nd - 1].ss == int64_t(es) && dims[nd - 1].ds == int64_t(ed)) {
             m.inner = uint64_t(dims[nd - 1].size) * ed;
@@ -267,7 +266,8 @@ static inline float bf16_to_f32(uint16_t v) {
     std::memcpy(&f, &u, 4);
     return f;
 }
-// round-to-nearest-even, NaN -> 0x7FC0: what torch's CPU path produces (c10::BFloat16)
+// round-to-nearest-even (c10::BFloat16's rounding), NaN -> 0x7FC0.  torch's CPU path has no fixed NaN encoding: fp32 ->
+// bf16 writes 0xFFFF, fp64 -> bf16 0x7FC0 or 0xFFFF depending on whether its scalar or vectorised loop ran.
 static inline uint16_t f32_to_bf16(float f) {
     if (std::isnan(f)) return 0x7FC0;
     uint32_t u;
@@ -294,12 +294,13 @@ static inline uint8_t quantize_host(float x, double scale, int64_t zp, bool is_s
 }
 
 static inline void store_from(void* p, uint32_t dt, const void* sp, uint32_t sdt) {
-    // convert through float when the source is <= 32 bit (exact), through double otherwise
+    // convert through float when the source is <= 32 bit (exact), through double otherwise; fp64 -> fp16 rounds to fp32
+    // first, as torch does (c10::Half is only built from a float)
     if (sdt == TSNAP_F64) {
         double x;
         std::memcpy(&x, sp, 8);
         switch (dt) {
-            case TSNAP_F16: { _Float16 h = (_Float16)x; std::memcpy(p, &h, 2); break; }
+            case TSNAP_F16: { _Float16 h = (_Float16)float(x); std::memcpy(p, &h, 2); break; }
             case TSNAP_BF16: { uint16_t v = f32_to_bf16(float(x)); std::memcpy(p, &v, 2); break; }
             case TSNAP_F32: { float f = float(x); std::memcpy(p, &f, 4); break; }
             default: std::memcpy(p, &x, 8);
