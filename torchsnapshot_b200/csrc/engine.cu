@@ -551,10 +551,24 @@ void tsnap_engine::put_table(void* p, size_t cap) {
     tbl_free.emplace_back(cap, p);
 }
 
-static void push_pending(tsnap_engine* eng, cudaEvent_t ev, std::function<void(bool)> fn) {
+// The two ways a job hands out asynchronous work: a task for the I/O workers (to `queue`, -1 = any) and an entry the
+// completion thread runs once `ev` has completed.  Each holds a part of the job from hand-out until it has run.
+static void post_io(tsnap_job* job, std::function<void()> fn, int queue = -1) {
+    job->hold();
+    job->eng->io->post([job, fn = std::move(fn)] {
+        fn();
+        job->part_done();
+    }, queue);
+}
+static void post_pending(tsnap_job* job, cudaEvent_t ev, std::function<void(bool)> fn) {
+    tsnap_engine* eng = job->eng;
+    job->hold();
     {
         std::lock_guard<std::mutex> g(eng->c_mu);
-        eng->pending.push_back({ev, std::move(fn)});
+        eng->pending.push_back({ev, [job, fn = std::move(fn)](bool ok) {
+                                    fn(ok);
+                                    job->part_done();
+                                }});
     }
     eng->c_cv.notify_one();
 }
@@ -723,6 +737,15 @@ static void collect_wave_timing(tsnap_job* job, Wave& w) {
     }
     job->stats.kernel_ms += total;
     w.kernel_ms = total;
+}
+
+// gives the wave's launch table back to the pool and destroys its events: its kernels and copies have finished
+static void release_wave(tsnap_engine* eng, Wave& w) {
+    if (w.d_tables) eng->put_table(w.d_tables, w.table_cap);
+    for (cudaEvent_t ev : w.ev_bucket)
+        if (ev) cudaEventDestroy(ev);
+    if (w.ev_done) cudaEventDestroy(w.ev_done);
+    if (w.ev_copied) cudaEventDestroy(w.ev_copied);
 }
 
 // What a job asks of the HBM staging arena.
@@ -934,7 +957,6 @@ static void finish_file_part(tsnap_job* job, FileSpec& f, uint64_t bytes_io, boo
             f.fd = -1;
         }
     }
-    job->part_done();
 }
 
 // Files are opened by the worker that performs their first I/O and closed by the one that performs the last:
@@ -963,7 +985,7 @@ static bool ensure_open(tsnap_job* job, FileSpec& f, bool save) {
         job->fail(TSNAP_EIO, "open " + f.path + ": " + strerror(errno));
         return false;
     }
-    if (job->eng->trace) job->add_trace(TSNAP_TR_OPEN, g_lane, int(&f - &job->files[0]), t0, job->now_ms(), 0);
+    if (job->eng->trace) job->add_trace(TSNAP_TR_OPEN, g_lane, f.index, t0, job->now_ms(), 0);
     return true;
 }
 
@@ -1021,7 +1043,7 @@ static void post_host_file(tsnap_job* job, int fi, bool save) {
     const uint64_t sb = eng->ring.slot_bytes();
     if (f.nbytes == 0) {
         if (save)
-            eng->io->post([job, &f] {
+            post_io(job, [job, &f] {
                 ensure_open(job, f, true);
                 finish_file_part(job, f, 0, true);
             });
@@ -1029,7 +1051,7 @@ static void post_host_file(tsnap_job* job, int fi, bool save) {
     }
     Member dm;
     if (save && direct_host_member(f, save, &dm)) {
-        eng->io->post([job, &f, dm, sb] {
+        post_io(job, [job, &f, dm, sb] {
             if (!job->failed() && ensure_open(job, f, true)) {
                 for (uint64_t lo = 0; lo < f.nbytes && !job->failed(); lo += sb) {
                     const uint64_t n = std::min<uint64_t>(sb, f.nbytes - lo);
@@ -1044,7 +1066,7 @@ static void post_host_file(tsnap_job* job, int fi, bool save) {
     if (direct_host_member(f, save, &dm)) {
         for (uint64_t lo = 0; lo < f.nbytes; lo += sb) {
             const uint64_t n = std::min(sb, f.nbytes - lo);
-            eng->io->post([job, &f, dm, lo, n] {
+            post_io(job, [job, &f, dm, lo, n] {
                 if (!job->failed() && ensure_open(job, f, false)) {
                     if (pread_all(f.fd, reinterpret_cast<char*>(uintptr_t(dm.dst)) + lo, n, f.offset + lo) != 0)
                         job->fail(TSNAP_EIO, "pread " + f.path + ": " + strerror(errno));
@@ -1054,7 +1076,7 @@ static void post_host_file(tsnap_job* job, int fi, bool save) {
         }
         return;
     }
-    eng->io->post([job, &f, save] {
+    post_io(job, [job, &f, save] {
         if (!job->failed() && ensure_open(job, f, save)) {
             char* tmp = static_cast<char*>(malloc(f.nbytes));
             if (!tmp) {
@@ -1101,16 +1123,21 @@ static void mark_device_done(tsnap_job* job) {
     }
 }
 
-// parts_left = asynchronous parts + 1: the extra token belongs to the drain thread, which drops it when
-// it no longer touches the job (run_job).  Waiters may destroy the job the moment the count hits zero.
-static void account_parts(tsnap_job* job, int64_t async_parts) {
-    job->parts_left.store(async_parts + 1);
-    job->accounted = true;
-}
-
-// chunk I/O goes to the queue of the NUMA node the pinned slot lives on (node-affine workers, see io_worker_specs)
-static void post_slot(tsnap_engine* eng, char* slot, std::function<void()> fn) {
-    eng->io->post(std::move(fn), eng->ring.queue_of(slot));
+// Retires wave wi's kernels (pack on save and stage, scatter on load; the uploads of a direct load wave): fails the
+// job on a kernel error or a NaN / Inf channel, collects and traces the kernel time, and with `gate` marks the
+// device side done.
+static void arm_wave_done(tsnap_job* job, size_t wi, bool gate) {
+    Wave* w = &job->waves[wi];
+    post_pending(job, w->ev_done, [job, w, wi, gate](bool ok) {
+        if (!ok) job->fail(TSNAP_ECUDA, job->kind == kLoad ? "scatter kernel failed" : "pack kernel failed");
+        check_nonfinite(job);
+        collect_wave_timing(job, *w);
+        if (job->eng->trace && !w->direct) {
+            const double t1 = job->now_ms();
+            job->add_trace(TSNAP_TR_KERNEL, int(wi), -1, t1 - w->kernel_ms, t1, w->bytes);
+        }
+        if (gate) mark_device_done(job);
+    });
 }
 
 // payload memcpys of chunk [lo, lo+n) of a direct file: one per dense run that intersects it
@@ -1128,6 +1155,43 @@ static bool direct_chunk_copies(tsnap_job* job, const FileSpec& f, char* slot, u
         job->n_memcpy.fetch_add(1, std::memory_order_relaxed);
     }
     return ok;
+}
+
+// Copies chunk [lo, lo+n) of file f between a pinned slot and the device on s_copy: the wave's arena region, or the
+// live tensors of a direct wave.  A failed job only records the event, so that the chunk still retires in order.
+// `then` runs on the completion thread once the copy has finished.
+static void issue_chunk_copy(tsnap_job* job, const Wave& w, FileSpec& f, char* slot, uint64_t lo, uint64_t n, bool to_host,
+                             std::function<void()> then) {
+    tsnap_engine* eng = job->eng;
+    cudaEvent_t ev = eng->get_event();
+    const double t_issue = eng->trace ? job->now_ms() : 0;
+    bool ok = true;
+    if (!job->failed()) {
+        if (w.direct) {
+            ok = direct_chunk_copies(job, f, slot, lo, n, to_host);
+        } else {
+            char* dev = job->arena + w.region_off + f.arena_off + lo;
+            ok = (to_host ? cudaMemcpyAsync(slot, dev, n, cudaMemcpyDeviceToHost, eng->s_copy)
+                          : cudaMemcpyAsync(dev, slot, n, cudaMemcpyHostToDevice, eng->s_copy)) == cudaSuccess;
+            job->n_memcpy.fetch_add(1, std::memory_order_relaxed);
+        }
+    }
+    ok = ok && cudaEventRecord(ev, eng->s_copy) == cudaSuccess;
+    const std::string dir = to_host ? "D2H" : "H2D";
+    if (!ok) job->fail(TSNAP_ECUDA, dir + " copy: " + cudaGetErrorString(cudaGetLastError()));
+    (to_host ? eng->bytes_d2h : eng->bytes_h2d) += n;
+    post_pending(job, ev, [job, ev, fi = f.index, n, t_issue, to_host, dir, then = std::move(then)](bool evok) {
+        job->eng->put_event(ev);
+        if (!evok) job->fail(TSNAP_ECUDA, dir + " copy failed");
+        if (job->eng->trace) {
+            // the copy engine runs the chunks of s_copy back to back: busy since the later of "issued" and
+            // "previous chunk done"
+            const double t1 = job->now_ms();
+            job->add_trace(to_host ? TSNAP_TR_D2H : TSNAP_TR_H2D, 0, fi, std::max(t_issue, job->last_copy_done_ms), t1, n);
+            job->last_copy_done_ms = t1;
+        }
+        then();
+    });
 }
 
 // the planning of a save or load job: the ring, the waves, and the member and tile tables of every wave
@@ -1153,77 +1217,45 @@ static int run_save_inner(tsnap_job* job) {
     tsnap_engine* eng = job->eng;
     int rc = plan_job(job);
     if (rc != TSNAP_OK) return rc;
-    // The first waves' pack kernels go out before anything else: they run while the rest of the job is set up,
-    // which keeps the async_take blocking window at plan + pack.  Nothing asynchronous references the job yet,
-    // so a failure below only has to drain the stream before returning.
     const size_t nw = job->waves.size();
     const size_t ns = job->n_staged_waves;
     const bool has_direct = nw > ns;
-    size_t launched = 0;
-    if (job->ev_producer && ns > 0) CUDA_TRY(cudaStreamWaitEvent(eng->s_kernel, job->ev_producer, 0));
-    for (; launched < std::min<size_t>(2, ns); ++launched) {
-        rc = launch_wave(job, job->waves[launched]);
-        if (rc != TSNAP_OK) {
-            cudaStreamSynchronize(eng->s_kernel);
-            return rc;
-        }
-    }
-    auto bail = [&](int code) {
-        std::string msg = last_err();
-        cudaStreamSynchronize(eng->s_kernel);
-        return set_err(code, msg);
-    };
-    // part count of every file before anything can complete (files are opened by the workers, see ensure_open)
-    int64_t parts = 0;
-    for (FileSpec& f : job->files) {
-        const int64_t p = count_parts(eng, f, true);
-        f.parts_left.store(p);
-        parts += p;
-    }
-    for (Wave& w : job->waves)
-        if (cudaEventCreateWithFlags(&w.ev_copied, cudaEventDisableTiming) != cudaSuccess) return bail(set_err(TSNAP_ECUDA, "event create failed"));
-    if (nw > 0) {
-        if (cudaEventCreate(&job->ev_copy_begin) != cudaSuccess || cudaEventCreate(&job->ev_copy_end) != cudaSuccess)
-            return bail(set_err(TSNAP_ECUDA, "event create failed"));
-    }
-    // the "direct copies finished" notification is retired by the completion thread AFTER the wave's chunk entries, i.e.
-    // possibly after the last write: it keeps the job alive with a part of its own
-    if (has_direct) parts += 1;
-    account_parts(job, parts);
-    if (nw == 0) mark_device_done(job);
-    if (parts == 0) return TSNAP_OK;
-
     // Sources are reusable (the async_take gate) once the last pack kernel has finished and, when files are drained
     // straight from the live tensors, once the last of those copies has finished.
     // (a wave that quantises per channel is always armed: its entry fails the job before any chunk of the wave is
     // written when a channel held a NaN or Inf — the completion thread retires entries in order)
-    auto arm_kernel_done = [&](Wave& w, size_t wi, bool gate) {
-        Wave* wp = &w;
-        push_pending(eng, w.ev_done, [job, wp, wi, gate, eng](bool ok) {
-            if (!ok) job->fail(TSNAP_ECUDA, "pack kernel failed");
-            check_nonfinite(job);
-            if (eng->trace) {
-                collect_wave_timing(job, *wp);
-                const double t1 = job->now_ms();
-                job->add_trace(TSNAP_TR_KERNEL, int(wi), -1, t1 - wp->kernel_ms, t1, wp->bytes);
-            }
-            if (gate) mark_device_done(job);
-        });
-    };
-    for (size_t wi = 0; wi < launched; ++wi) {
-        const bool gate = !has_direct && wi + 1 == ns;
-        if (gate || eng->trace || job->waves[wi].qkey_bytes) arm_kernel_done(job->waves[wi], wi, gate);
-    }
+    size_t launched = 0;
     auto launch_next = [&]() -> int {
         Wave& w = job->waves[launched];
         if (launched >= 2) CUDA_TRY(cudaStreamWaitEvent(eng->s_kernel, job->waves[launched - 2].ev_copied, 0));
         int r = launch_wave(job, w);
         if (r != TSNAP_OK) return r;
         const bool gate = !has_direct && launched + 1 == ns;
-        if (gate || eng->trace || w.qkey_bytes) arm_kernel_done(w, launched, gate);
+        if (gate || eng->trace || w.qkey_bytes) arm_wave_done(job, launched, gate);
         ++launched;
         return TSNAP_OK;
     };
+    // The first waves' pack kernels go out before anything else: they run while the rest of the job is set up,
+    // which keeps the async_take blocking window at plan + pack.  Until the chunks are issued, a failure only has
+    // to drain the stream before returning.
+    auto bail = [&](int code) {
+        std::string msg = last_err();
+        cudaStreamSynchronize(eng->s_kernel);
+        return set_err(code, msg);
+    };
+    if (job->ev_producer && ns > 0) CUDA_TRY(cudaStreamWaitEvent(eng->s_kernel, job->ev_producer, 0));
+    while (launched < std::min<size_t>(2, ns))
+        if ((rc = launch_next()) != TSNAP_OK) return bail(rc);
+    // part count of every file before anything can complete (files are opened by the workers, see ensure_open)
+    for (FileSpec& f : job->files) f.parts_left.store(count_parts(eng, f, true));
+    for (Wave& w : job->waves)
+        if (cudaEventCreateWithFlags(&w.ev_copied, cudaEventDisableTiming) != cudaSuccess) return bail(set_err(TSNAP_ECUDA, "event create failed"));
+    if (nw > 0) {
+        if (cudaEventCreate(&job->ev_copy_begin) != cudaSuccess || cudaEventCreate(&job->ev_copy_end) != cudaSuccess)
+            return bail(set_err(TSNAP_ECUDA, "event create failed"));
+    }
+    if (nw == 0) mark_device_done(job);
+
     // host-only files go straight to the I/O workers
     for (size_t i = 0; i < job->files.size(); ++i) {
         FileSpec& f = job->files[i];
@@ -1235,6 +1267,7 @@ static int run_save_inner(tsnap_job* job) {
         bool ok;
         if (w.direct) ok = !job->ev_producer || cudaStreamWaitEvent(eng->s_copy, job->ev_producer, 0) == cudaSuccess;
         else ok = cudaStreamWaitEvent(eng->s_copy, w.ev_done, 0) == cudaSuccess;
+        if (!ok) job->fail(TSNAP_ECUDA, std::string("D2H copy: ") + cudaGetErrorString(cudaGetLastError()));
         if (wi == 0) cudaEventRecord(job->ev_copy_begin, eng->s_copy);
         // Buffered writes take the inode lock exclusively, so two chunks of one file never make progress at
         // the same time.  Treat every file as a sequential job and spread its chunks evenly over the whole
@@ -1266,73 +1299,37 @@ static int run_save_inner(tsnap_job* job) {
             if (link_idle) job->link_starved_us += int64_t(waited * 1000.0);
             job->copies_in_flight.fetch_add(1, std::memory_order_acq_rel);
             if (eng->trace && waited > 0.05) job->add_trace(TSNAP_TR_SLOT_WAIT, 0, cr.fi, tw_ms, job->now_ms(), 0);
-            cudaEvent_t ev = eng->get_event();
-            const double t_issue = eng->trace ? job->now_ms() : 0;
-            if (ok && !job->failed()) {
-                if (w.direct) {
-                    ok = direct_chunk_copies(job, f, slot, lo, n, true);
-                } else {
-                    ok = cudaMemcpyAsync(slot, job->arena + w.region_off + f.arena_off + lo, n, cudaMemcpyDeviceToHost, eng->s_copy) == cudaSuccess;
-                    job->n_memcpy.fetch_add(1, std::memory_order_relaxed);
-                }
-            }
-            ok = ok && cudaEventRecord(ev, eng->s_copy) == cudaSuccess;
-            if (!ok) job->fail(TSNAP_ECUDA, std::string("D2H copy: ") + cudaGetErrorString(cudaGetLastError()));
-            eng->bytes_d2h += n;
-            FileSpec* fp = &f;
-            const int fidx = cr.fi;
-            push_pending(eng, ev, [eng, job, fp, fidx, slot, lo, n, ev, t_issue](bool evok) {
-                eng->put_event(ev);
+            // the write goes to the queue of the NUMA node the pinned slot lives on (node-affine workers, see io_worker_specs)
+            issue_chunk_copy(job, w, f, slot, lo, n, true, [job, &f, slot, lo, n] {
                 job->copies_in_flight.fetch_sub(1, std::memory_order_acq_rel);
-                if (!evok) job->fail(TSNAP_ECUDA, "D2H copy failed");
-                if (eng->trace) {
-                    // the copy engine runs the chunks of s_copy back to back: busy since the later of "issued" and
-                    // "previous chunk done"
-                    const double t1 = job->now_ms();
-                    job->add_trace(TSNAP_TR_D2H, 0, fidx, std::max(t_issue, job->last_copy_done_ms), t1, n);
-                    job->last_copy_done_ms = t1;
-                }
                 auto tq = clk::now();
-                post_slot(eng, slot, [eng, job, fp, fidx, slot, lo, n, tq] {
+                post_io(job, [job, &f, slot, lo, n, tq] {
                     job->io_queue_us += int64_t(ms_since(tq) * 1000.0);
                     NvtxRange nvtx_w("tsnap:pwrite chunk");
-                    if (!job->failed() && ensure_open(job, *fp, true)) {
+                    if (!job->failed() && ensure_open(job, f, true)) {
                         auto tb = clk::now();
-                        const double t0w = eng->trace ? job->now_ms() : 0;
+                        const double t0w = job->eng->trace ? job->now_ms() : 0;
                         {
                             TokenGuard tok;
-                            if (write_chunk(*fp, slot, n, lo) != 0) job->fail(TSNAP_EIO, "pwrite " + fp->path + ": " + strerror(errno));
+                            if (write_chunk(f, slot, n, lo) != 0) job->fail(TSNAP_EIO, "pwrite " + f.path + ": " + strerror(errno));
                         }
                         job->io_busy_us += int64_t(ms_since(tb) * 1000.0);
-                        if (eng->trace) job->add_trace(TSNAP_TR_PWRITE, g_lane, fidx, t0w, job->now_ms(), n);
+                        if (job->eng->trace) job->add_trace(TSNAP_TR_PWRITE, g_lane, f.index, t0w, job->now_ms(), n);
                     }
                     job->give_slot(slot);
-                    finish_file_part(job, *fp, n, true);
-                });
+                    finish_file_part(job, f, n, true);
+                }, job->eng->ring.queue_of(slot));
             });
         }
         if (wi + 1 == nw) cudaEventRecord(job->ev_copy_end, eng->s_copy);
         if (cudaEventRecord(w.ev_copied, eng->s_copy) != cudaSuccess) job->fail(TSNAP_ECUDA, "event record failed");
-        if (w.direct)  // (this entry is queued behind the wave's chunk entries: it holds a part of its own, see below)
-            push_pending(eng, w.ev_copied, [job](bool evok) {
+        if (w.direct)  // queued behind the wave's chunk entries
+            post_pending(job, w.ev_copied, [job](bool evok) {
                 if (!evok) job->fail(TSNAP_ECUDA, "D2H copy failed");
                 mark_device_done(job);
-                job->part_done();
             });
-        if (launched < ns) {
-            rc = launch_next();
-            if (rc != TSNAP_OK) {
-                job->fail(rc, last_err());
-                mark_device_done(job);
-                // remaining waves are never issued
-                int64_t remaining = 0;
-                for (size_t wj = wi + 1; wj < nw; ++wj)
-                    for (int fj : job->waves[wj].files) remaining += job->files[fj].parts_left.load();
-                if (has_direct) remaining += 1;  // the direct wave's completion entry is never queued either
-                for (int64_t i = 0; i < remaining; ++i) job->part_done();
-                return TSNAP_OK;
-            }
-        }
+        // a launch failure leaves the later waves unissued: they hold no part of the job
+        if (launched < ns && (rc = launch_next()) != TSNAP_OK) return rc;
     }
     return TSNAP_OK;
 }
@@ -1350,19 +1347,7 @@ static int run_load_inner(tsnap_job* job) {
     int rc = plan_job(job);
     if (rc != TSNAP_OK) return rc;
     const uint64_t sb = eng->ring.slot_bytes();
-    int64_t parts = 0;
-    for (FileSpec& f : job->files) {
-        if (f.nbytes == 0) continue;
-        const int64_t p = count_parts(eng, f, false);
-        f.parts_left.store(p);
-        parts += p;
-    }
-    parts += int64_t(job->waves.size());  // one part per wave for its scatter kernels
-    account_parts(job, parts);
-    if (parts == 0) {
-        mark_device_done(job);
-        return TSNAP_OK;
-    }
+    for (FileSpec& f : job->files) f.parts_left.store(count_parts(eng, f, false));
     for (Wave& w : job->waves) {
         int64_t c = 0;
         for (int fi : w.files) c += int64_t((job->files[fi].nbytes + sb - 1) / sb);
@@ -1399,57 +1384,28 @@ static int run_load_inner(tsnap_job* job) {
         const bool last_wave = (wi + 1 == nw);
         for (int fi : w->files) {
             FileSpec* f = &job->files[fi];
-            char* base = w->direct ? nullptr : job->arena + w->region_off + f->arena_off;
             for (uint64_t lo = 0; lo < f->nbytes; lo += sb) {
                 const uint64_t n = std::min(sb, f->nbytes - lo);
                 char* slot = job->take_slot();
-                post_slot(eng, slot, [eng, job, w, wi, f, fi, base, slot, lo, n, shared, last_wave] {
+                post_io(job, [eng, job, w, wi, f, slot, lo, n, shared, last_wave] {
                     NvtxRange nvtx_r("tsnap:pread chunk + H2D enqueue");
                     cudaSetDevice(eng->device);
-                    bool ok = !job->failed();
+                    const bool ok = !job->failed();
                     uint64_t skip = 0;
                     const double t0r = eng->trace ? job->now_ms() : 0;
                     if (ok && f->mem_src) {
                         memcpy(slot, f->mem_src + lo, n);
                     } else if (ok) {
                         auto tb = clk::now();
-                        if (!ensure_open(job, *f, false)) {
-                            ok = false;
-                        } else {
+                        if (ensure_open(job, *f, false)) {
                             TokenGuard tok;
-                            if (read_chunk(*f, slot, n, f->offset + lo, &skip) != 0) {
+                            if (read_chunk(*f, slot, n, f->offset + lo, &skip) != 0)
                                 job->fail(TSNAP_EIO, "pread " + f->path + ": " + strerror(errno));
-                                ok = false;
-                            }
                         }
                         job->io_busy_us += int64_t(ms_since(tb) * 1000.0);
                     }
-                    const double t_issue = eng->trace ? job->now_ms() : 0;
-                    if (eng->trace) job->add_trace(TSNAP_TR_PREAD, g_lane, fi, t0r, t_issue, n);
-                    cudaEvent_t ev = eng->get_event();
-                    if (ok) {
-                        bool cok;
-                        if (w->direct) {
-                            cok = direct_chunk_copies(job, *f, slot + skip, lo, n, false);
-                        } else {
-                            cok = cudaMemcpyAsync(base + lo, slot + skip, n, cudaMemcpyHostToDevice, eng->s_copy) == cudaSuccess;
-                            job->n_memcpy.fetch_add(1, std::memory_order_relaxed);
-                        }
-                        if (!cok) {
-                            job->fail(TSNAP_ECUDA, "H2D copy failed to enqueue");
-                            ok = false;
-                        }
-                    }
-                    cudaEventRecord(ev, eng->s_copy);
-                    eng->bytes_h2d += n;
-                    push_pending(eng, ev, [eng, job, f, fi, slot, n, ev, t_issue](bool evok) {
-                        eng->put_event(ev);
-                        if (!evok) job->fail(TSNAP_ECUDA, "H2D copy failed");
-                        if (eng->trace) {
-                            const double t1 = job->now_ms();
-                            job->add_trace(TSNAP_TR_H2D, 0, fi, std::max(t_issue, job->last_copy_done_ms), t1, n);
-                            job->last_copy_done_ms = t1;
-                        }
+                    if (eng->trace) job->add_trace(TSNAP_TR_PREAD, g_lane, f->index, t0r, job->now_ms(), n);
+                    issue_chunk_copy(job, *w, *f, slot + skip, lo, n, false, [job, f, slot, n] {
                         job->give_slot(slot);
                         finish_file_part(job, *f, n, false);
                     });
@@ -1474,23 +1430,10 @@ static int run_load_inner(tsnap_job* job) {
                             shared->launched[wi] = 1;
                         }
                         shared->cv.notify_all();
-                        if (r == TSNAP_OK && w->ev_done && !job->failed()) {
-                            push_pending(eng, w->ev_done, [eng, job, w, wi, last_wave](bool evok) {
-                                if (!evok) job->fail(TSNAP_ECUDA, "scatter kernel failed");
-                                collect_wave_timing(job, *w);
-                                if (eng->trace && !w->direct) {
-                                    const double t1 = job->now_ms();
-                                    job->add_trace(TSNAP_TR_KERNEL, int(wi), -1, t1 - w->kernel_ms, t1, w->bytes);
-                                }
-                                if (last_wave) mark_device_done(job);
-                                job->part_done();
-                            });
-                        } else {
-                            if (last_wave) mark_device_done(job);
-                            job->part_done();
-                        }
+                        if (r == TSNAP_OK && w->ev_done && !job->failed()) arm_wave_done(job, wi, last_wave);
+                        else if (last_wave) mark_device_done(job);
                     }
-                });
+                }, eng->ring.queue_of(slot));
             }
         }
     }
@@ -1517,7 +1460,6 @@ static int run_stage_inner(tsnap_job* job) {
         }
     }
     if (dev.empty() || f.nbytes == 0) {
-        account_parts(job, 0);
         mark_device_done(job);
         return TSNAP_OK;
     }
@@ -1536,7 +1478,6 @@ static int run_stage_inner(tsnap_job* job) {
     CUDA_TRY(cudaEventCreate(&job->ev_copy_begin));
     CUDA_TRY(cudaEventCreate(&job->ev_copy_end));
     char* out = static_cast<char*>(job->stage_buf);
-    Wave* wp = &w;
     if (w.direct) {
         // no HBM staging available: dense members go straight from the live tensors into the pinned buffer
         if (job->ev_producer) CUDA_TRY(cudaStreamWaitEvent(eng->s_copy, job->ev_producer, 0));
@@ -1572,19 +1513,11 @@ static int run_stage_inner(tsnap_job* job) {
     CUDA_TRY(cudaEventRecord(job->ev_copy_end, eng->s_copy));
     cudaEvent_t ev = eng->get_event();
     CUDA_TRY(cudaEventRecord(ev, eng->s_copy));
-    account_parts(job, 1);
-    if (!w.direct)
-        push_pending(eng, w.ev_done, [job](bool ok) {
-            if (!ok) job->fail(TSNAP_ECUDA, "pack kernel failed");
-            check_nonfinite(job);
-            mark_device_done(job);
-        });
-    push_pending(eng, ev, [eng, job, ev, wp](bool ok) {
-        eng->put_event(ev);
+    if (!w.direct) arm_wave_done(job, 0, true);
+    post_pending(job, ev, [job, ev](bool ok) {
+        job->eng->put_event(ev);
         if (!ok) job->fail(TSNAP_ECUDA, "D2H copy failed");
-        collect_wave_timing(job, *wp);
         mark_device_done(job);
-        job->part_done();
     });
     return TSNAP_OK;
 }
@@ -1609,10 +1542,6 @@ static void run_job(tsnap_job* job) {
     if (rc != TSNAP_OK) {
         job->fail(rc, last_err());
         mark_device_done(job);
-        if (!job->accounted) {
-            // failed before any asynchronous part was handed out
-            account_parts(job, 0);
-        }
     }
     job->part_done();  // the drain thread's token: `job` may be destroyed by a waiter from here on
 }
@@ -1850,7 +1779,8 @@ static int add_file(tsnap_job* job, const char* path, uint64_t offset, uint64_t 
     f.offset = offset;
     f.nbytes = nbytes;
     f.dense = true;
-    *idx = int32_t(job->files.size()) - 1;
+    f.index = int(job->files.size()) - 1;
+    *idx = f.index;
     return TSNAP_OK;
 }
 int tsnap_save_job_add_file(tsnap_job* job, const char* path, uint64_t nbytes, int32_t* file_index) {
@@ -1958,6 +1888,7 @@ static int submit(tsnap_job* job, void* stream, bool is_consumer) {
         }
     }
     job->submitted = true;
+    job->parts_left.store(1);  // the drain thread's token: run_job drops it when it no longer touches the job
     job->t_submit = clk::now();
     eng->active_jobs.fetch_add(1, std::memory_order_acq_rel);
     {
@@ -2038,13 +1969,7 @@ int tsnap_job_destroy(tsnap_job* job) {
         job->cv.wait(g, [job] { return job->done; });
     }
     if (job->eng->has_device) cudaSetDevice(job->eng->device);
-    for (Wave& w : job->waves) {
-        if (w.d_tables) job->eng->put_table(w.d_tables, w.table_cap);  // the job is done: its kernels have finished
-        for (cudaEvent_t ev : w.ev_bucket)
-            if (ev) cudaEventDestroy(ev);
-        if (w.ev_done) cudaEventDestroy(w.ev_done);
-        if (w.ev_copied) cudaEventDestroy(w.ev_copied);
-    }
+    for (Wave& w : job->waves) release_wave(job->eng, w);  // the job is done: its kernels have finished
     if (job->ev_producer) cudaEventDestroy(job->ev_producer);
     if (job->ev_consumer) cudaEventDestroy(job->ev_consumer);
     if (job->ev_copy_begin) cudaEventDestroy(job->ev_copy_begin);
@@ -2359,18 +2284,16 @@ int tsnap_scatter_device(tsnap_engine* eng, const void* device_wire, uint64_t nb
     job.kind = kLoad;
     job.arena = static_cast<char*>(const_cast<void*>(device_wire));
     job.arena_bytes = nbytes;
-    job.files.emplace_back();
-    FileSpec& f = job.files.back();
-    f.path = "<device wire>";
-    f.nbytes = nbytes;
+    int32_t fi;
+    add_file(&job, "<device wire>", 0, nbytes, &fi);
     for (int32_t i = 0; i < n; ++i) {
         if (members[i].src_space != TSNAP_SPACE_WIRE || members[i].dst_space != TSNAP_SPACE_DEVICE)
             return set_err(TSNAP_EINVAL, "scatter_device members go from WIRE to DEVICE");
-        int rc = add_member(&job, 0, &members[i], false);
+        int rc = add_member(&job, fi, &members[i], false);
         if (rc != TSNAP_OK) return rc;
     }
     Wave w;
-    w.files.push_back(0);
+    w.files.push_back(fi);
     int rc = plan_wave(&job, w);
     if (rc != TSNAP_OK) return rc;
     cudaEvent_t ev = eng->get_event();
@@ -2380,13 +2303,8 @@ int tsnap_scatter_device(tsnap_engine* eng, const void* device_wire, uint64_t nb
     if (e != cudaSuccess) return set_err(TSNAP_ECUDA, std::string("scatter_device: ") + cudaGetErrorString(e));
     rc = launch_wave(&job, w);
     if (rc == TSNAP_OK && cudaEventSynchronize(w.ev_done) != cudaSuccess) rc = set_err(TSNAP_ECUDA, "scatter kernel failed");
-    if (w.d_tables) {
-        if (rc != TSNAP_OK) cudaStreamSynchronize(eng->s_kernel);
-        eng->put_table(w.d_tables, w.table_cap);
-    }
-    for (cudaEvent_t x : w.ev_bucket)
-        if (x) cudaEventDestroy(x);
-    if (w.ev_done) cudaEventDestroy(w.ev_done);
+    if (rc != TSNAP_OK) cudaStreamSynchronize(eng->s_kernel);
+    release_wave(eng, w);
     return rc;
 }
 

@@ -152,17 +152,11 @@ struct FileSpec {
     int fd = -1;
     bool opened = false, open_failed = false, direct_io = false;
     std::mutex open_mu;
-    std::atomic<int64_t> parts_left{0};
+    std::atomic<int64_t> parts_left{0};  // I/O parts not yet finished: the last one closes the file
     uint64_t arena_off = 0;  // offset inside the wave's arena region
     int wave = -1;
+    int index = -1;                 // position in the job's files (trace records)
     const char* mem_src = nullptr;  // load: the "file" is caller memory (consumer seam)
-    FileSpec() = default;
-    FileSpec(const FileSpec& o)
-        : path(o.path), offset(o.offset), nbytes(o.nbytes), members(o.members), host_only(o.host_only), dense(o.dense),
-          direct(o.direct), segs(o.segs), fd(o.fd), opened(o.opened), open_failed(o.open_failed), direct_io(o.direct_io),
-          arena_off(o.arena_off), wave(o.wave), mem_src(o.mem_src) {
-        parts_left.store(o.parts_left.load());
-    }
 };
 
 struct Wave {
@@ -192,7 +186,7 @@ enum JobKind { kSave = 0, kLoad = 1, kStage = 2 };
 struct tsnap_job {
     tsnap_engine* eng = nullptr;
     int kind = tsnap::kSave;
-    std::vector<tsnap::FileSpec> files;
+    std::deque<tsnap::FileSpec> files;
     std::deque<tsnap::Wave> waves;   // staged waves first, then at most one direct pseudo-wave
     size_t n_staged_waves = 0;
     cudaEvent_t ev_producer = nullptr;
@@ -211,7 +205,6 @@ struct tsnap_job {
     double last_copy_done_ms = 0;  // completion thread only
     void add_trace(int kind, int lane, int file, double t0, double t1, uint64_t bytes);
     double now_ms() const { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_submit).count(); }
-    bool accounted = false;  // parts_left (incl. the drain thread's own token) has been set
     // completion state
     std::mutex mu;
     std::condition_variable cv;
@@ -219,6 +212,8 @@ struct tsnap_job {
     bool done = false;
     int err_code = 0;
     std::string err_msg;
+    // outstanding work: the drain thread's token (set at submit) plus one part per task handed out and not yet
+    // finished.  A task is handed out only by a holder of a part, so the count reaches zero once, when all is done.
     std::atomic<int64_t> parts_left{0};
     // per-channel descriptors: the job's own copies of their tsnap_qchannel records (the caller's are only read during
     // add_member), and the host-mapped word the parameter kernel raises on a NaN / Inf channel
@@ -243,6 +238,7 @@ struct tsnap_job {
 
     void fail(int code, const std::string& msg);
     bool failed();
+    void hold() { parts_left.fetch_add(1, std::memory_order_relaxed); }
     void part_done();
 };
 
