@@ -456,6 +456,9 @@ static inline uint64_t align_up(uint64_t x, uint64_t a) { return (x + a - 1) / a
 using namespace tsnap;
 
 // ---- job plumbing -----------------------------------------------------------------------------------------
+// where the tensor side of a member lives: its source on save, its destination on load
+static int tensor_space(const tsnap_job* job, const tsnap_copy_desc& d) { return job->kind == kLoad ? d.dst_space : d.src_space; }
+
 void tsnap_job::fail(int code, const std::string& msg) {
     std::lock_guard<std::mutex> g(mu);
     if (err_code == 0) {
@@ -618,6 +621,7 @@ static int plan_wave(tsnap_job* job, Wave& w) {
         FileSpec& f = job->files[fi];
         const uint64_t wire_base = uint64_t(uintptr_t(job->arena)) + w.region_off + f.arena_off;
         for (const tsnap_copy_desc& d : f.members) {
+            if (tensor_space(job, d) == TSNAP_SPACE_HOST) continue;  // a mixed sink's host members: see post_host_file
             NormalizedCopy nc;
             int rc = normalize_copy(d, wire_base, true, &nc, &err);
             if (rc != TSNAP_OK) return set_err(rc, "member of " + f.path + ": " + err);
@@ -754,13 +758,12 @@ struct ArenaNeed {
     uint64_t nd_total = 0, nd_largest = 0;    // files that cannot be drained without staging (strided / cast members)
 };
 // A device file is one with a member whose tensor side is DEVICE.  The test needs no submit (tsnap_job_arena_hint runs
-// before it); afterwards it equals !host_only, because submit rejects files that mix HOST and DEVICE members.
+// before it); afterwards it equals !host_only.
 static ArenaNeed arena_need(const tsnap_job* job) {
     ArenaNeed n;
     for (const FileSpec& f : job->files) {
         bool device = false;
-        for (const tsnap_copy_desc& d : f.members)
-            device = device || (job->kind == kLoad ? d.dst_space : d.src_space) == TSNAP_SPACE_DEVICE;
+        for (const tsnap_copy_desc& d : f.members) device = device || tensor_space(job, d) == TSNAP_SPACE_DEVICE;
         if (!device || f.nbytes == 0) continue;
         const uint64_t fb = align_up(f.nbytes, 256);
         n.total += fb;
@@ -862,9 +865,10 @@ static int build_waves(tsnap_job* job) {
     for (size_t i = 0; i < job->files.size(); ++i) {
         FileSpec& f = job->files[i];
         if (f.host_only || f.nbytes == 0) continue;
-        if (f.dense && !stage_dense) {
-            f.direct = true;
+        f.direct = f.dense && !stage_dense;
+        if (f.direct || f.mixed)  // copied segment by segment (extent_copies)
             std::sort(f.segs.begin(), f.segs.end(), [](const FileSpec::Seg& x, const FileSpec::Seg& y) { return x.off < y.off; });
+        if (f.direct) {
             direct_files.push_back(int(i));
             job->stats.direct_bytes += f.nbytes;
             continue;
@@ -1023,26 +1027,50 @@ static int read_chunk(FileSpec& f, char* slot, uint64_t n, uint64_t off, uint64_
     return 0;
 }
 
+// bytes per chunk of a device file: a ring slot, or the whole of a memory sink (it needs no slot)
+static uint64_t chunk_bytes(tsnap_engine* eng, const FileSpec& f) {
+    return f.mem_dst ? f.nbytes : eng->ring.slot_bytes();
+}
+
 // number of I/O parts a file contributes
 static int64_t count_parts(tsnap_engine* eng, const FileSpec& f, bool save) {
     if (f.nbytes == 0) return save ? 1 : 0;  // an empty file still has to be created on save
-    const uint64_t sb = eng->ring.slot_bytes();
     if (f.host_only) {
+        const uint64_t sb = eng->ring.slot_bytes();
         Member m;
         // direct reads run in parallel parts (shared inode lock); direct writes of one file are one sequential
         // part: buffered writes serialise on the inode lock anyway, parallel parts only add contention
         if (!save && direct_host_member(f, save, &m)) return int64_t((f.nbytes + sb - 1) / sb);
         return 1;
     }
-    return int64_t((f.nbytes + sb - 1) / sb);
+    const uint64_t cb = chunk_bytes(eng, f);
+    return int64_t((f.nbytes + cb - 1) / cb);
 }
 
+// copies the HOST members of f between their tensors and the wire image at `wire`; false when one failed the job
+static bool copy_host_members(tsnap_job* job, const FileSpec& f, char* wire) {
+    std::string err;
+    for (const tsnap_copy_desc& d : f.members) {
+        if (tensor_space(job, d) != TSNAP_SPACE_HOST) continue;  // a mixed sink's device members
+        NormalizedCopy nc;
+        int rc = normalize_copy(d, uint64_t(uintptr_t(wire)), false, &nc, &err);
+        if (rc == TSNAP_OK) rc = host_copy_all(nc, &err);
+        if (rc != TSNAP_OK) {
+            job->fail(rc, "member of " + f.path + ": " + err);
+            return false;
+        }
+    }
+    return true;
+}
+
+// The host members of file fi.  A memory sink's are copied into it right here, on the calling thread; every other
+// file's are read or written by the I/O workers.
 static void post_host_file(tsnap_job* job, int fi, bool save) {
     tsnap_engine* eng = job->eng;
     FileSpec& f = job->files[fi];
     const uint64_t sb = eng->ring.slot_bytes();
     if (f.nbytes == 0) {
-        if (save)
+        if (save && !f.mem_dst)
             post_io(job, [job, &f] {
                 ensure_open(job, f, true);
                 finish_file_part(job, f, 0, true);
@@ -1050,6 +1078,11 @@ static void post_host_file(tsnap_job* job, int fi, bool save) {
         return;
     }
     Member dm;
+    if (f.mem_dst) {  // the sink is the wire image itself: no slab, no write
+        if (direct_host_member(f, true, &dm)) memcpy(f.mem_dst, reinterpret_cast<const char*>(uintptr_t(dm.src)), f.nbytes);
+        else copy_host_members(job, f, f.mem_dst);
+        return;
+    }
     if (save && direct_host_member(f, save, &dm)) {
         post_io(job, [job, &f, dm, sb] {
             if (!job->failed() && ensure_open(job, f, true)) {
@@ -1082,22 +1115,12 @@ static void post_host_file(tsnap_job* job, int fi, bool save) {
             if (!tmp) {
                 job->fail(TSNAP_ENOMEM, "malloc of a host slab failed");
             } else {
-                std::string err;
                 bool ok = true;
                 if (!save && pread_all(f.fd, tmp, f.nbytes, f.offset) != 0) {
                     job->fail(TSNAP_EIO, "pread " + f.path + ": " + strerror(errno));
                     ok = false;
                 }
-                for (size_t i = 0; ok && i < f.members.size(); ++i) {
-                    NormalizedCopy nc;
-                    int rc = normalize_copy(f.members[i], uint64_t(uintptr_t(tmp)), false, &nc, &err);
-                    if (rc == TSNAP_OK) rc = host_copy_all(nc, &err);
-                    if (rc != TSNAP_OK) {
-                        job->fail(rc, "member of " + f.path + ": " + err);
-                        ok = false;
-                        break;
-                    }
-                }
+                ok = ok && copy_host_members(job, f, tmp);
                 if (ok && save && pwrite_all(f.fd, tmp, f.nbytes, 0) != 0)
                     job->fail(TSNAP_EIO, "pwrite " + f.path + ": " + strerror(errno));
                 free(tmp);
@@ -1123,7 +1146,7 @@ static void mark_device_done(tsnap_job* job) {
     }
 }
 
-// Retires wave wi's kernels (pack on save and stage, scatter on load; the uploads of a direct load wave): fails the
+// Retires wave wi's kernels (pack on save, scatter on load; the uploads of a direct load wave): fails the
 // job on a kernel error or a NaN / Inf channel, collects and traces the kernel time, and with `gate` marks the
 // device side done.
 static void arm_wave_done(tsnap_job* job, size_t wi, bool gate) {
@@ -1140,8 +1163,10 @@ static void arm_wave_done(tsnap_job* job, size_t wi, bool gate) {
     });
 }
 
-// payload memcpys of chunk [lo, lo+n) of a direct file: one per dense run that intersects it
-static bool direct_chunk_copies(tsnap_job* job, const FileSpec& f, char* slot, uint64_t lo, uint64_t n, bool to_host) {
+// payload memcpys of chunk [lo, lo+n) of a file copied segment by segment (FileSpec::segs): one per segment that
+// intersects it, from / to its dense run in the live tensors (`region` null) or its bytes in the wave's arena region
+static bool extent_copies(tsnap_job* job, const FileSpec& f, char* slot, char* region, uint64_t lo, uint64_t n, bool to_host,
+                          uint64_t* copied) {
     tsnap_engine* eng = job->eng;
     size_t i = size_t(std::upper_bound(f.segs.begin(), f.segs.end(), lo, [](uint64_t v, const FileSpec::Seg& s) { return v < s.off + s.bytes; }) - f.segs.begin());
     bool ok = true;
@@ -1149,37 +1174,42 @@ static bool direct_chunk_copies(tsnap_job* job, const FileSpec& f, char* slot, u
         const FileSpec::Seg& sg = f.segs[i];
         const uint64_t a = std::max(lo, sg.off), b = std::min(lo + n, sg.off + sg.bytes);
         if (a >= b) continue;
-        char* dev = reinterpret_cast<char*>(uintptr_t(sg.addr)) + (a - sg.off);
+        char* dev = region ? region + a : reinterpret_cast<char*>(uintptr_t(sg.addr)) + (a - sg.off);
         ok = to_host ? cudaMemcpyAsync(slot + (a - lo), dev, b - a, cudaMemcpyDeviceToHost, eng->s_copy) == cudaSuccess
                      : cudaMemcpyAsync(dev, slot + (a - lo), b - a, cudaMemcpyHostToDevice, eng->s_copy) == cudaSuccess;
         job->n_memcpy.fetch_add(1, std::memory_order_relaxed);
+        *copied += b - a;
     }
     return ok;
 }
 
-// Copies chunk [lo, lo+n) of file f between a pinned slot and the device on s_copy: the wave's arena region, or the
-// live tensors of a direct wave.  A failed job only records the event, so that the chunk still retires in order.
-// `then` runs on the completion thread once the copy has finished.
+// Copies chunk [lo, lo+n) of file f between a pinned slot (or memory sink) and the device on s_copy: the wave's arena
+// region, or the live tensors of a direct wave; a mixed sink moves only its device members' extents.  A failed job
+// only records the event, so that the chunk still retires in order.  `then` runs on the completion thread once the
+// copy has finished.
 static void issue_chunk_copy(tsnap_job* job, const Wave& w, FileSpec& f, char* slot, uint64_t lo, uint64_t n, bool to_host,
                              std::function<void()> then) {
     tsnap_engine* eng = job->eng;
     cudaEvent_t ev = eng->get_event();
     const double t_issue = eng->trace ? job->now_ms() : 0;
     bool ok = true;
+    uint64_t copied = 0;
     if (!job->failed()) {
-        if (w.direct) {
-            ok = direct_chunk_copies(job, f, slot, lo, n, to_host);
+        char* region = w.direct ? nullptr : job->arena + w.region_off + f.arena_off;
+        if (w.direct || f.mixed) {
+            ok = extent_copies(job, f, slot, region, lo, n, to_host, &copied);
         } else {
-            char* dev = job->arena + w.region_off + f.arena_off + lo;
-            ok = (to_host ? cudaMemcpyAsync(slot, dev, n, cudaMemcpyDeviceToHost, eng->s_copy)
-                          : cudaMemcpyAsync(dev, slot, n, cudaMemcpyHostToDevice, eng->s_copy)) == cudaSuccess;
+            ok = (to_host ? cudaMemcpyAsync(slot, region + lo, n, cudaMemcpyDeviceToHost, eng->s_copy)
+                          : cudaMemcpyAsync(region + lo, slot, n, cudaMemcpyHostToDevice, eng->s_copy)) == cudaSuccess;
             job->n_memcpy.fetch_add(1, std::memory_order_relaxed);
+            copied = n;
         }
     }
     ok = ok && cudaEventRecord(ev, eng->s_copy) == cudaSuccess;
     const std::string dir = to_host ? "D2H" : "H2D";
     if (!ok) job->fail(TSNAP_ECUDA, dir + " copy: " + cudaGetErrorString(cudaGetLastError()));
-    (to_host ? eng->bytes_d2h : eng->bytes_h2d) += n;
+    // a memory sink counts the bytes it moved, a file chunk its whole length
+    (to_host ? eng->bytes_d2h : eng->bytes_h2d) += f.mem_dst ? copied : n;
     post_pending(job, ev, [job, ev, fi = f.index, n, t_issue, to_host, dir, then = std::move(then)](bool evok) {
         job->eng->put_event(ev);
         if (!evok) job->fail(TSNAP_ECUDA, dir + " copy failed");
@@ -1197,7 +1227,10 @@ static void issue_chunk_copy(tsnap_job* job, const Wave& w, FileSpec& f, char* s
 // the planning of a save or load job: the ring, the waves, and the member and tile tables of every wave
 static int plan_job(tsnap_job* job) {
     tsnap_engine* eng = job->eng;
-    int rc = ensure_ring(eng);
+    // every file but a memory sink moves through ring slots or in pieces of their size: a job of sinks alone (the
+    // stager seam) does not make the engine allocate its ring
+    const bool ring = std::any_of(job->files.begin(), job->files.end(), [](const FileSpec& f) { return !f.mem_dst; });
+    int rc = ring ? ensure_ring(eng) : TSNAP_OK;
     if (rc != TSNAP_OK) return rc;
     auto t0 = clk::now();
     const double tr0 = job->now_ms();
@@ -1215,6 +1248,9 @@ static int plan_job(tsnap_job* job) {
 static int run_save_inner(tsnap_job* job) {
     NvtxRange nvtx_job("tsnap:save_job issue (plan, pack launch, D2H issue)");
     tsnap_engine* eng = job->eng;
+    // a memory sink's host members are copied before any device work: they have been read when the device side is done
+    for (size_t i = 0; i < job->files.size(); ++i)
+        if (job->files[i].mem_dst && (job->files[i].host_only || job->files[i].mixed)) post_host_file(job, int(i), true);
     int rc = plan_job(job);
     if (rc != TSNAP_OK) return rc;
     const size_t nw = job->waves.size();
@@ -1259,9 +1295,8 @@ static int run_save_inner(tsnap_job* job) {
     // host-only files go straight to the I/O workers
     for (size_t i = 0; i < job->files.size(); ++i) {
         FileSpec& f = job->files[i];
-        if (f.host_only || f.nbytes == 0) post_host_file(job, int(i), true);
+        if (!f.mem_dst && (f.host_only || f.nbytes == 0)) post_host_file(job, int(i), true);
     }
-    const uint64_t sb = eng->ring.slot_bytes();
     for (size_t wi = 0; wi < nw; ++wi) {
         Wave& w = job->waves[wi];
         bool ok;
@@ -1281,15 +1316,19 @@ static int run_save_inner(tsnap_job* job) {
         };
         std::vector<ChunkRef> order;
         for (int fi : w.files) {
-            const uint64_t nb = job->files[fi].nbytes;
-            const uint64_t c = (nb + sb - 1) / sb;
-            for (uint64_t k = 0; k < c; ++k) order.push_back({fi, k * sb, (double(k) + 0.5) / double(c)});
+            const uint64_t nb = job->files[fi].nbytes, cb = chunk_bytes(eng, job->files[fi]);
+            const uint64_t c = (nb + cb - 1) / cb;
+            for (uint64_t k = 0; k < c; ++k) order.push_back({fi, k * cb, (double(k) + 0.5) / double(c)});
         }
         std::stable_sort(order.begin(), order.end(), [](const ChunkRef& x, const ChunkRef& y) { return x.due < y.due; });
         for (const ChunkRef& cr : order) {
             FileSpec& f = job->files[cr.fi];
             const uint64_t lo = cr.lo;
-            const uint64_t n = std::min(sb, f.nbytes - lo);
+            const uint64_t n = std::min(chunk_bytes(eng, f), f.nbytes - lo);
+            if (f.mem_dst) {  // the chunk lands in the sink: no slot, no write
+                issue_chunk_copy(job, w, f, f.mem_dst + lo, lo, n, true, [job, &f] { finish_file_part(job, f, 0, true); });
+                continue;
+            }
             auto tw = clk::now();
             const double tw_ms = eng->trace ? job->now_ms() : 0;
             const bool link_idle = job->copies_in_flight.load(std::memory_order_acquire) == 0;
@@ -1441,93 +1480,12 @@ static int run_load_inner(tsnap_job* job) {
     return TSNAP_OK;
 }
 
-// ---- stage (whole-buffer pinned sink) ---------------------------------------------------------------------
-static int run_stage_inner(tsnap_job* job) {
-    tsnap_engine* eng = job->eng;
-    FileSpec& f = job->files[0];
-    auto t0 = clk::now();
-    // host members are copied right here; device members go through the pack kernels
-    std::vector<tsnap_copy_desc> dev;
-    std::string err;
-    for (const tsnap_copy_desc& d : f.members) {
-        if (d.src_space == TSNAP_SPACE_HOST) {
-            NormalizedCopy nc;
-            int rc = normalize_copy(d, uint64_t(uintptr_t(job->stage_buf)), false, &nc, &err);
-            if (rc == TSNAP_OK) rc = host_copy_all(nc, &err);
-            if (rc != TSNAP_OK) return set_err(rc, err);
-        } else {
-            dev.push_back(d);
-        }
-    }
-    if (dev.empty() || f.nbytes == 0) {
-        mark_device_done(job);
-        return TSNAP_OK;
-    }
-    if (!eng->has_device) return set_err(TSNAP_ECUDA, "device members on a host-only engine");
-    // device members may be interleaved with host members; pack into the arena image of the whole
-    // buffer and copy back only the spans that device members cover (here: the whole buffer when no
-    // host member exists, else per-member spans)
-    const bool mixed = dev.size() != f.members.size();
-    f.members = dev;
-    int rc = build_waves(job);
-    if (rc != TSNAP_OK) return rc;
-    Wave& w = job->waves[0];
-    rc = plan_wave(job, w);
-    if (rc != TSNAP_OK) return rc;
-    job->stats.plan_ms = ms_since(t0);
-    CUDA_TRY(cudaEventCreate(&job->ev_copy_begin));
-    CUDA_TRY(cudaEventCreate(&job->ev_copy_end));
-    char* out = static_cast<char*>(job->stage_buf);
-    if (w.direct) {
-        // no HBM staging available: dense members go straight from the live tensors into the pinned buffer
-        if (job->ev_producer) CUDA_TRY(cudaStreamWaitEvent(eng->s_copy, job->ev_producer, 0));
-        CUDA_TRY(cudaEventRecord(job->ev_copy_begin, eng->s_copy));
-        for (const FileSpec::Seg& sg : f.segs) {
-            CUDA_TRY(cudaMemcpyAsync(out + sg.off, reinterpret_cast<const void*>(uintptr_t(sg.addr)), sg.bytes, cudaMemcpyDeviceToHost, eng->s_copy));
-            eng->bytes_d2h += sg.bytes;
-            job->n_memcpy.fetch_add(1, std::memory_order_relaxed);
-        }
-    } else {
-        if (job->ev_producer) CUDA_TRY(cudaStreamWaitEvent(eng->s_kernel, job->ev_producer, 0));
-        rc = launch_wave(job, w);
-        if (rc != TSNAP_OK) return rc;
-        CUDA_TRY(cudaStreamWaitEvent(eng->s_copy, w.ev_done, 0));
-        CUDA_TRY(cudaEventRecord(job->ev_copy_begin, eng->s_copy));
-        const char* base = job->arena + w.region_off + f.arena_off;
-        if (!mixed) {
-            CUDA_TRY(cudaMemcpyAsync(out, base, f.nbytes, cudaMemcpyDeviceToHost, eng->s_copy));
-            eng->bytes_d2h += f.nbytes;
-            job->n_memcpy.fetch_add(1, std::memory_order_relaxed);
-        } else {
-            for (const tsnap_copy_desc& d : dev) {
-                uint64_t numel = 1;
-                for (int i = 0; i < d.ndim; ++i) numel *= uint64_t(d.sizes[i]);
-                const uint64_t nb = numel * dtype_size(d.dst_dtype);
-                if (nb == 0) continue;
-                CUDA_TRY(cudaMemcpyAsync(out + d.dst_addr, base + d.dst_addr, nb, cudaMemcpyDeviceToHost, eng->s_copy));
-                eng->bytes_d2h += nb;
-                job->n_memcpy.fetch_add(1, std::memory_order_relaxed);
-            }
-        }
-    }
-    CUDA_TRY(cudaEventRecord(job->ev_copy_end, eng->s_copy));
-    cudaEvent_t ev = eng->get_event();
-    CUDA_TRY(cudaEventRecord(ev, eng->s_copy));
-    if (!w.direct) arm_wave_done(job, 0, true);
-    post_pending(job, ev, [job, ev](bool ok) {
-        job->eng->put_event(ev);
-        if (!ok) job->fail(TSNAP_ECUDA, "D2H copy failed");
-        mark_device_done(job);
-    });
-    return TSNAP_OK;
-}
-
 static void run_job(tsnap_job* job) {
     tsnap_engine* eng = job->eng;
     if (eng->has_device) cudaSetDevice(eng->device);
     // Jobs are issued back to back, but the staging arena (and its two wave regions) belongs to one device job
     // at a time: a job that touches the GPU waits here until its predecessor has completely drained.
-    bool device_job = job->kind == kStage;
+    bool device_job = false;
     for (const FileSpec& f : job->files) device_job = device_job || (!f.host_only && f.nbytes > 0);
     if (device_job && eng->has_device && !job->arena_set && !eng->no_arena) {
         std::unique_lock<std::mutex> ga(eng->arena_mu);
@@ -1535,10 +1493,7 @@ static void run_job(tsnap_job* job) {
         eng->arena_in_use = true;
         job->holds_arena = true;
     }
-    int rc;
-    if (job->kind == kSave) rc = run_save_inner(job);
-    else if (job->kind == kLoad) rc = run_load_inner(job);
-    else rc = run_stage_inner(job);
+    const int rc = job->kind == kSave ? run_save_inner(job) : run_load_inner(job);
     if (rc != TSNAP_OK) {
         job->fail(rc, last_err());
         mark_device_done(job);
@@ -1808,15 +1763,22 @@ static int add_member(tsnap_job* job, int32_t fi, const tsnap_copy_desc* d, bool
     uint64_t numel = 1;
     for (int i = 0; i < d->ndim; ++i) numel *= uint64_t(d->sizes[i]);
     tsnap_copy_desc own = *d;
+    // save: the member's extent on the wire — its elements and the per-tensor trailer of a quantising copy, or the
+    // per-channel header (8 bytes in front of the body), body and parameters
+    uint64_t wire_lo = d->dst_addr, wire_end = 0;
     if (d->reserved == TSNAP_QSCHEME_PER_CHANNEL) {
         // the engine plans after this call returns: keep its own copy of the record
         if (nc.qc.params + 16 * nc.qc.channels > f.nbytes) return set_err(TSNAP_EINVAL, "per-channel parameters exceed the file's wire image");
         job->qrecs.push_back(*reinterpret_cast<const tsnap_qchannel*>(uintptr_t(d->q_zero_point)));
         own.q_zero_point = int64_t(uintptr_t(&job->qrecs.back()));
+        if (save) {
+            wire_lo = nc.qc.body - 8;
+            wire_end = nc.qc.params + 16 * nc.qc.channels;
+        }
     } else if (save) {
         const bool quant = d->dst_dtype == TSNAP_QINT8 || d->dst_dtype == TSNAP_QUINT8;
-        const uint64_t end = d->dst_addr + numel * dtype_size(d->dst_dtype) + (quant && numel ? 16 : 0);
-        if (end > f.nbytes) return set_err(TSNAP_EINVAL, "member exceeds the file's wire image");
+        wire_end = d->dst_addr + numel * dtype_size(d->dst_dtype) + (quant && numel ? 16 : 0);
+        if (wire_end > f.nbytes) return set_err(TSNAP_EINVAL, "member exceeds the file's wire image");
     } else if (numel) {
         // furthest byte touched on the wire side
         uint64_t last = d->src_addr;
@@ -1824,13 +1786,13 @@ static int add_member(tsnap_job* job, int32_t fi, const tsnap_copy_desc* d, bool
             last += uint64_t(d->sizes[i] - 1) * uint64_t(d->src_strides[i]) * dtype_size(d->src_dtype);
         if (last + dtype_size(d->src_dtype) > f.nbytes) return set_err(TSNAP_EINVAL, "member reads past the byte range");
     }
-    // dense, cast-free device members can be drained / uploaded without staging: remember their runs
-    const int tensor_space = save ? d->src_space : d->dst_space;
-    if (numel && tensor_space == TSNAP_SPACE_DEVICE) {
-        if (nc.n == 1 && nc.m[0].mode == kModeContig)
-            f.segs.push_back(FileSpec::Seg{save ? nc.m[0].dst : nc.m[0].src, save ? nc.m[0].src : nc.m[0].dst, nc.m[0].bytes});
-        else
-            f.dense = false;
+    // dense, cast-free device members can be drained / uploaded without staging: remember their runs (and on save
+    // every other device member's extent; a run's extent is the run)
+    if (numel && (save ? d->src_space : d->dst_space) == TSNAP_SPACE_DEVICE) {
+        const bool run = nc.n == 1 && nc.m[0].mode == kModeContig;
+        if (save) f.segs.push_back(FileSpec::Seg{wire_lo, run ? nc.m[0].src : 0, wire_end - wire_lo});
+        else if (run) f.segs.push_back(FileSpec::Seg{nc.m[0].src, nc.m[0].dst, nc.m[0].bytes});
+        f.dense = f.dense && run;
     }
     f.members.push_back(own);
     job->stats.n_members++;
@@ -1851,26 +1813,15 @@ static int submit(tsnap_job* job, void* stream, bool is_consumer) {
     bool any_device = false;
     for (FileSpec& f : job->files) {
         job->stats.payload_bytes += f.nbytes;
-        bool host = true;
-        for (const tsnap_copy_desc& d : f.members) {
-            const int sp = job->kind == kLoad ? d.dst_space : d.src_space;
-            if (sp != TSNAP_SPACE_HOST) host = false;
-        }
-        if (job->kind == kStage) {
-            f.host_only = false;
-            any_device = any_device || !host;
-            continue;
-        }
-        if (!host) {
-            for (const tsnap_copy_desc& d : f.members) {
-                const int sp = job->kind == kLoad ? d.dst_space : d.src_space;
-                if (sp == TSNAP_SPACE_HOST)
-                    return set_err(TSNAP_EUNSUP, "a file mixes HOST and DEVICE members: " + f.path +
-                                                     " (the batcher keeps CPU and GPU slabs apart, T:batcher.py:300-303)");
-            }
-        }
-        f.host_only = host;
-        any_device = any_device || !host;
+        bool host = false, device = false;
+        for (const tsnap_copy_desc& d : f.members) (tensor_space(job, d) == TSNAP_SPACE_HOST ? host : device) = true;
+        // only a memory sink takes both: its host members are copied into it, its device members' extents copied back
+        if (host && device && !f.mem_dst)
+            return set_err(TSNAP_EUNSUP, "a file mixes HOST and DEVICE members: " + f.path +
+                                             " (the batcher keeps CPU and GPU slabs apart, T:batcher.py:300-303)");
+        f.host_only = !device;
+        f.mixed = host && device;
+        any_device = any_device || device;
     }
     if (any_device && !eng->has_device) return set_err(TSNAP_ECUDA, "device members on a host-only engine");
     if (any_device && !is_consumer) {
@@ -2152,7 +2103,7 @@ int tsnap_stage_submit(tsnap_engine* eng, const tsnap_copy_desc* members, int32_
                        void* producer_stream, tsnap_buffer** out) {
     if (!eng || !out || (n > 0 && !members)) return set_err(TSNAP_EINVAL, "null argument");
     tsnap_job* job = nullptr;
-    int rc = job_create(eng, kStage, &job);
+    int rc = job_create(eng, kSave, &job);
     if (rc != TSNAP_OK) return rc;
     int32_t fi;
     add_file(job, "<stage>", 0, nbytes, &fi);
@@ -2167,20 +2118,21 @@ int tsnap_stage_submit(tsnap_engine* eng, const tsnap_copy_desc* members, int32_
             return rc;
         }
     }
-    job->stage_buf = pin_get(eng, nbytes, &job->stage_cap);
-    if (!job->stage_buf) {
+    size_t cap = 0;
+    char* buf = static_cast<char*>(pin_get(eng, nbytes, &cap));
+    if (!buf) {
         delete job;
         return set_err(TSNAP_ENOMEM, "pinned allocation failed");
     }
+    job->files[0].mem_dst = buf;
     rc = submit(job, producer_stream, false);
     if (rc != TSNAP_OK) {
         std::lock_guard<std::mutex> g(eng->pin_mu);
-        eng->pin_cache.emplace_back(job->stage_cap, job->stage_buf);
+        eng->pin_cache.emplace_back(cap, buf);
         delete job;
         return rc;
     }
-    tsnap_buffer* b = new tsnap_buffer{job};
-    *out = b;
+    *out = new tsnap_buffer{job, buf, cap};
     return TSNAP_OK;
 }
 int tsnap_buffer_wait_device(tsnap_buffer* buf) {
@@ -2190,7 +2142,7 @@ int tsnap_buffer_wait_device(tsnap_buffer* buf) {
 int tsnap_buffer_wait(tsnap_buffer* buf, void** host_ptr, uint64_t* nbytes) {
     if (!buf) return set_err(TSNAP_EINVAL, "null buffer");
     int rc = tsnap_job_wait(buf->job);
-    if (host_ptr) *host_ptr = buf->job->stage_buf;
+    if (host_ptr) *host_ptr = buf->stage_buf;
     if (nbytes) *nbytes = buf->job->files[0].nbytes;
     return rc;
 }
@@ -2208,7 +2160,7 @@ int tsnap_buffer_release(tsnap_buffer* buf) {
     }
     {
         std::lock_guard<std::mutex> g(eng->pin_mu);
-        eng->pin_cache.emplace_back(job->stage_cap, job->stage_buf);
+        eng->pin_cache.emplace_back(buf->stage_cap, buf->stage_buf);
         // keep the cache bounded: drop the largest buffers beyond 8 entries
         while (eng->pin_cache.size() > 8) {
             size_t big = 0;

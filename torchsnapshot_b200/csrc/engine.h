@@ -143,9 +143,13 @@ struct FileSpec {
     uint64_t nbytes = 0;
     std::vector<tsnap_copy_desc> members;
     bool host_only = false;  // every member lives in HOST space
-    bool dense = false;      // every member is one dense, cast-free run: can be drained without staging
+    bool mixed = false;      // a memory sink with HOST and DEVICE members
+    bool dense = false;      // every device member is one dense, cast-free run: can be drained without staging
     bool direct = false;     // chosen for this job: D2H straight from the live tensors (no arena, no pack)
-    struct Seg {             // dense runs of a dense file: wire offset, tensor-side address, length
+    // Device members on the wire: offset, tensor-side address of a dense run (else 0), length.  Save records every
+    // device member's whole extent (quantisation trailer, per-channel header and parameters included); load only
+    // the dense runs.  A direct file copies its runs one by one; a mixed sink copies back only these extents.
+    struct Seg {
         uint64_t off, addr, bytes;
     };
     std::vector<Seg> segs;
@@ -157,6 +161,7 @@ struct FileSpec {
     int wave = -1;
     int index = -1;                 // position in the job's files (trace records)
     const char* mem_src = nullptr;  // load: the "file" is caller memory (consumer seam)
+    char* mem_dst = nullptr;        // save: the "file" is this pinned host buffer (stager seam)
 };
 
 struct Wave {
@@ -179,7 +184,7 @@ struct Wave {
     std::atomic<int64_t> chunks_to_upload{0};                         // load: H2D chunks not yet issued
 };
 
-enum JobKind { kSave = 0, kLoad = 1, kStage = 2 };
+enum JobKind { kSave = 0, kLoad = 1 };
 
 }  // namespace tsnap
 
@@ -219,9 +224,6 @@ struct tsnap_job {
     // add_member), and the host-mapped word the parameter kernel raises on a NaN / Inf channel
     std::deque<tsnap_qchannel> qrecs;
     int* qflag = nullptr;
-    // stager seam (kStage): whole-buffer pinned sink
-    void* stage_buf = nullptr;
-    size_t stage_cap = 0;
     // stats
     tsnap_job_stats stats{};
     bool timing_collected = false;
@@ -242,6 +244,9 @@ struct tsnap_job {
     void part_done();
 };
 
+// stager seam: a save job whose one file is a pinned block of the pin cache
 struct tsnap_buffer {
     tsnap_job* job;
+    char* stage_buf;
+    size_t stage_cap;
 };
