@@ -37,8 +37,9 @@ extern "C" {
 #define TSNAP_ESTATE (-5)   /* call made in the wrong job state              */
 #define TSNAP_EUNSUP (-6)   /* dtype pair / layout not supported             */
 
-/* element types: the ten buffer-protocol dtypes of T:serialization.py:162-173 (raw path).  The
- * enum value only selects element size and, when src_dtype != dst_dtype, the conversion. */
+/* element types: the ten buffer-protocol dtypes of T:serialization.py:162-173 (raw path), the two quantised wire
+ * types and the two plain float8 formats.  The enum value only selects element size and, when src_dtype != dst_dtype,
+ * the conversion. */
 enum tsnap_dtype {
     TSNAP_U8 = 0,   /* torch.uint8 / torch.bool (1-byte payload, copied verbatim) */
     TSNAP_I8 = 1,
@@ -56,7 +57,12 @@ enum tsnap_dtype {
      * (T:serialization.py:278-310) — the north star's "quantize in the pack kernel". */
     TSNAP_QINT8 = 10,
     TSNAP_QUINT8 = 11,
-    TSNAP_DTYPE_COUNT = 12
+    /* torch.float8_e4m3fn / torch.float8_e5m2 (OCP FP8, 1-byte raw images).  Converted to and from F16 / BF16 / F32 /
+     * F64 and each other with torch's rounding (through fp32, round to nearest even, subnormals kept; e4m3fn turns
+     * values past 464 and +-inf into NaN with the sign kept, e5m2 overflows to +-inf).  Not a quantisation source. */
+    TSNAP_F8E4M3FN = 12,
+    TSNAP_F8E5M2 = 13,
+    TSNAP_DTYPE_COUNT = 14
 };
 
 /* where a side of a copy lives */

@@ -1,10 +1,11 @@
 """Isolated launches of every kernel mode through the C-ABI stager seam, for ncu captures and CUDA-event roofline
 numbers:  dense (bulk/TMA), column shard (rows/TMA), odd-alignment slab member (LSU contig), transpose (LSU tiled),
-fp32->bf16 cast (LSU cast), short strided runs (LSU strided), per-channel int8 quantisation (statistics + parameters +
-quantising pack) along dim 0 and dim 1, and its dequantising scatter.  Prints one JSON line per case with the kernel's
+fp32->bf16, fp32->e4m3fn and bf16->e4m3fn casts (LSU cast), short strided runs (LSU strided), per-channel int8 quantisation (statistics + parameters +
+quantising pack) along dim 0 and dim 1, its dequantising scatter, and an e4m3fn -> bf16 converting scatter.  Prints one JSON line per case with the kernel's
 CUDA-event time and achieved GB/s against the measured HBM copy peak (MEASURED_PEAKS.json; else the H100 SXM data
 sheet's 3.35 TB/s).  A per-channel save reads its source twice (statistics, then the pack): its algorithmic bytes are
-both reads, the 1-byte elements written and the 16 bytes of parameters per channel.
+both reads, the 1-byte elements written and the 16 bytes of parameters per channel; a cast's are the source and
+destination element sizes per element.
 
     python tools/kernel_cases.py [--case NAME] [--reps N]
     ncu --set full --clock-control none --import-source on -k regex:tsnap -o kernels python tools/kernel_cases.py --reps 1
@@ -37,6 +38,9 @@ def cases():
     hb = base.view(torch.bfloat16)[: 16384 * 8192].view(16384, 8192).t()
     yield "transpose_bf16_16384x8192", [(hb, 0, None)], hb.numel() * 2, 2 * hb.numel() * 2
     yield "cast_fp32_to_bf16_1GiB", [(base, 0, torch.bfloat16)], GiB // 2, GiB + GiB // 2
+    yield "cast_fp32_to_e4m3fn_1GiB", [(base, 0, torch.float8_e4m3fn)], GiB // 4, GiB + GiB // 4
+    hb = base.view(torch.bfloat16)
+    yield "cast_bf16_to_e4m3fn_1GiB", [(hb, 0, torch.float8_e4m3fn)], GiB // 2, GiB + GiB // 2
     short = base.view(1 << 22, 64)[:, 8:40]  # 128 B runs: below the copy-engine threshold
     yield "strided_128B_runs", [(short, 0, None)], short.numel() * 4, 2 * short.numel() * 4
     m = base.view(262144, 1024)
@@ -78,5 +82,20 @@ if args.case in ("all", "qchannel_dequant_fp32_axis0_1GiB"):
     ms = min(times)
     algo = dst.numel() + 16 * 262144 + dst.numel() * 4
     print(json.dumps({"case": "qchannel_dequant_fp32_axis0_1GiB", "kernel_ms": round(ms, 4), "note": "CUDA events around tsnap_scatter_device (table upload + launch + kernel)",
+                      "algorithmic_bytes": algo, "gbs": round(algo / 1e6 / ms, 1), "frac_of_measured_peak": round(algo / 1e6 / ms / peak, 3)}), flush=True)
+# converting scatter: a 1 GiB bf16 target from an e4m3fn image already in device memory
+if args.case in ("all", "scatter_e4m3fn_to_bf16_1GiB"):
+    dst = torch.empty(1 << 29, dtype=torch.bfloat16, device=dev)
+    wire = torch.empty(1 << 29, dtype=torch.float8_e4m3fn, device=dev).view(torch.uint8).random_(0, 256)
+    desc = N.load_desc(dst, 0, wire_dtype=torch.float8_e4m3fn)
+    ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
+    times = []
+    for rep in range(args.reps + 1):
+        ev[0].record(); eng.scatter_device(wire, [desc]); ev[1].record(); torch.cuda.synchronize()
+        if rep:
+            times.append(ev[0].elapsed_time(ev[1]))
+    ms = min(times)
+    algo = dst.numel() * 3
+    print(json.dumps({"case": "scatter_e4m3fn_to_bf16_1GiB", "kernel_ms": round(ms, 4), "note": "CUDA events around tsnap_scatter_device (table upload + launch + kernel)",
                       "algorithmic_bytes": algo, "gbs": round(algo / 1e6 / ms, 1), "frac_of_measured_peak": round(algo / 1e6 / ms / peak, 3)}), flush=True)
 eng.close()

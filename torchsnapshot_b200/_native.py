@@ -19,7 +19,7 @@ LIB_PATH = os.path.join(_HERE, "lib", "libtsnap_b200.so")
 MAX_DIMS = 8
 
 # enum tsnap_dtype
-U8, I8, I16, I32, I64, F16, BF16, F32, F64, BOOL, QINT8, QUINT8 = range(12)
+U8, I8, I16, I32, I64, F16, BF16, F32, F64, BOOL, QINT8, QUINT8, F8E4M3FN, F8E5M2 = range(14)
 # enum tsnap_space
 SPACE_DEVICE, SPACE_HOST, SPACE_WIRE = 0, 1, 2
 
@@ -31,7 +31,7 @@ ENGINE_NO_ARENA = 16
 PROBE_D2H, PROBE_H2D, PROBE_WRITE, PROBE_READ = 0, 1, 2, 3
 TRACE_KINDS = ("plan", "kernel", "d2h", "pwrite", "slot_wait", "pread", "h2d", "open")
 
-# the ten buffer-protocol dtypes of the reference (T:serialization.py:162-173)
+# the ten buffer-protocol dtypes of the reference (T:serialization.py:162-173) and the two float8 formats
 TORCH_TO_TSNAP = {
     torch.uint8: U8,
     torch.int8: I8,
@@ -43,6 +43,8 @@ TORCH_TO_TSNAP = {
     torch.float32: F32,
     torch.float64: F64,
     torch.bool: BOOL,
+    torch.float8_e4m3fn: F8E4M3FN,
+    torch.float8_e5m2: F8E5M2,
 }
 
 

@@ -17,6 +17,7 @@
 #include <cuda_fp16.h>
 #include <stdint.h>
 
+#include "fp8.h"
 #include "kernels.h"
 #include "ptx.cuh"
 
@@ -688,23 +689,31 @@ __device__ __forceinline__ uint64_t load_bits(const char* p, uint32_t n, bool al
 __device__ __forceinline__ void convert_store(char* p, uint32_t ddt, const char* sp, uint32_t sdt, bool src_aligned, bool aligned) {
     // <=32-bit float sources convert through fp32 (exact widening, with no detour through double: that would quiet the
     // signalling NaNs torch's bf16 -> fp32 widening keeps bit for bit).  fp64 sources narrow to fp32 and bf16 in one
-    // rounding step, and to fp16 through fp32: torch's copy kernel has no double -> half conversion (c10::Half is built
-    // from a float), so it rounds twice.
+    // rounding step, and to fp16 and float8 through fp32: torch's copy kernel has no double -> half or double -> float8
+    // conversion (c10::Half and c10::Float8_* are built from a float), so it rounds twice.  Float8 elements are single
+    // bytes: never misaligned.
     if (sdt == TSNAP_F64) {
         const double x = __longlong_as_double((long long)load_bits(sp, 8, src_aligned));
         if (ddt == TSNAP_F32) { const float f = (float)x; store_bytes(p, &f, 4, aligned); }
         else if (ddt == TSNAP_F16) { const __half h = __float2half_rn((float)x); store_bytes(p, &h, 2, aligned); }
         else if (ddt == TSNAP_BF16) { const __nv_bfloat16 b = __float2bfloat16_rn((float)x); store_bytes(p, &b, 2, aligned); }
+        else if (is_fp8_dtype(ddt)) *reinterpret_cast<uint8_t*>(p) = fp8_from_f32((float)x, ddt);
         else store_bytes(p, &x, 8, aligned);
         return;
     }
-    const uint32_t w = (uint32_t)load_bits(sp, sdt == TSNAP_F32 ? 4 : 2, src_aligned);
-    const float f = sdt == TSNAP_F32 ? __uint_as_float(w)
-                    : sdt == TSNAP_BF16 ? __bfloat162float(__ushort_as_bfloat16((unsigned short)w))
-                                        : __half2float(__ushort_as_half((unsigned short)w));
+    float f;
+    if (is_fp8_dtype(sdt)) {
+        f = fp8_to_f32(*reinterpret_cast<const uint8_t*>(sp), sdt);
+    } else {
+        const uint32_t w = (uint32_t)load_bits(sp, sdt == TSNAP_F32 ? 4 : 2, src_aligned);
+        f = sdt == TSNAP_F32 ? __uint_as_float(w)
+            : sdt == TSNAP_BF16 ? __bfloat162float(__ushort_as_bfloat16((unsigned short)w))
+                                : __half2float(__ushort_as_half((unsigned short)w));
+    }
     if (ddt == TSNAP_F32) store_bytes(p, &f, 4, aligned);
     else if (ddt == TSNAP_F16) { const __half h = __float2half_rn(f); store_bytes(p, &h, 2, aligned); }
     else if (ddt == TSNAP_BF16) { const __nv_bfloat16 b = __float2bfloat16_rn(f); store_bytes(p, &b, 2, aligned); }
+    else if (is_fp8_dtype(ddt)) *reinterpret_cast<uint8_t*>(p) = fp8_from_f32(f, ddt);
     else { const double x = (double)f; store_bytes(p, &x, 8, aligned); }
 }
 
@@ -752,6 +761,104 @@ __device__ __forceinline__ void cast_dense_vec(const char* __restrict__ s, char*
     }
 }
 
+// dense, 16 B aligned {fp32, bf16, fp16} <-> float8: 16 elements per thread, one 16 B access on the float8 side and
+// 16 B accesses on the wide side
+template <uint32_t kWide>
+__device__ __forceinline__ void ld16_as_f32(const char* s, float (&x)[16]) {
+    if (kWide == TSNAP_F32) {
+#pragma unroll
+        for (int v = 0; v < 4; ++v) {
+            const uint4 a = ld_stream16(s + 16 * v);
+            x[4 * v] = __uint_as_float(a.x);
+            x[4 * v + 1] = __uint_as_float(a.y);
+            x[4 * v + 2] = __uint_as_float(a.z);
+            x[4 * v + 3] = __uint_as_float(a.w);
+        }
+    } else {
+#pragma unroll
+        for (int v = 0; v < 2; ++v) {
+            const uint4 a = ld_stream16(s + 16 * v);
+            const uint32_t w[4] = {a.x, a.y, a.z, a.w};
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const float2 f = kWide == TSNAP_BF16 ? __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&w[i]))
+                                                     : __half22float2(*reinterpret_cast<const __half2*>(&w[i]));
+                x[8 * v + 2 * i] = f.x;
+                x[8 * v + 2 * i + 1] = f.y;
+            }
+        }
+    }
+}
+template <uint32_t kWide>
+__device__ __forceinline__ void st16_from_f32(char* d, const float (&x)[16]) {
+    if (kWide == TSNAP_F32) {
+#pragma unroll
+        for (int v = 0; v < 4; ++v)
+            st_stream16(d + 16 * v, make_uint4(__float_as_uint(x[4 * v]), __float_as_uint(x[4 * v + 1]), __float_as_uint(x[4 * v + 2]),
+                                               __float_as_uint(x[4 * v + 3])));
+    } else {
+#pragma unroll
+        for (int v = 0; v < 2; ++v) {
+            uint32_t o[4];
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                if (kWide == TSNAP_BF16) {
+                    const __nv_bfloat162 p = __floats2bfloat162_rn(x[8 * v + 2 * i], x[8 * v + 2 * i + 1]);
+                    o[i] = *reinterpret_cast<const uint32_t*>(&p);
+                } else {
+                    const __half2 p = __floats2half2_rn(x[8 * v + 2 * i], x[8 * v + 2 * i + 1]);
+                    o[i] = *reinterpret_cast<const uint32_t*>(&p);
+                }
+            }
+            st_stream16(d + 16 * v, make_uint4(o[0], o[1], o[2], o[3]));
+        }
+    }
+}
+template <bool kNarrow, uint32_t kWide, uint32_t kFp8>
+__device__ __forceinline__ void cast_fp8_vec(const char* __restrict__ s, char* __restrict__ d, uint64_t nelem) {
+    constexpr uint32_t kWideSize = kWide == TSNAP_F32 ? 4 : 2;
+    const uint64_t ngroups = nelem >> 4;
+    for (uint64_t g = threadIdx.x; g < ngroups; g += kLsuThreads) {
+        float x[16];
+        uint32_t o[4];
+        if (kNarrow) {
+            ld16_as_f32<kWide>(s + g * 16 * kWideSize, x);
+#pragma unroll
+            for (int i = 0; i < 4; ++i)
+                o[i] = (uint32_t)fp8_from_f32(x[4 * i], kFp8) | ((uint32_t)fp8_from_f32(x[4 * i + 1], kFp8) << 8) |
+                       ((uint32_t)fp8_from_f32(x[4 * i + 2], kFp8) << 16) | ((uint32_t)fp8_from_f32(x[4 * i + 3], kFp8) << 24);
+            st_stream16(d + g * 16, make_uint4(o[0], o[1], o[2], o[3]));
+        } else {
+            const uint4 a = ld_stream16(s + g * 16);
+            o[0] = a.x, o[1] = a.y, o[2] = a.z, o[3] = a.w;
+#pragma unroll
+            for (int i = 0; i < 16; ++i) x[i] = fp8_to_f32((uint8_t)(o[i >> 2] >> (8 * (i & 3))), kFp8);
+            st16_from_f32<kWide>(d + g * 16 * kWideSize, x);
+        }
+    }
+}
+template <bool kNarrow, uint32_t kWide>
+__device__ __forceinline__ void cast_fp8_vec_of(uint32_t fp8, const char* s, char* d, uint64_t nelem) {
+    if (fp8 == TSNAP_F8E4M3FN) cast_fp8_vec<kNarrow, kWide, TSNAP_F8E4M3FN>(s, d, nelem);
+    else cast_fp8_vec<kNarrow, kWide, TSNAP_F8E5M2>(s, d, nelem);
+}
+// the float8 vector path for (src, dst), if it has one: the number of elements it converted (a multiple of 16)
+__device__ __forceinline__ uint64_t cast_fp8_dense(uint32_t sdt, uint32_t ddt, const char* s, char* d, uint64_t nelem) {
+    const bool narrow = is_fp8_dtype(ddt);
+    const uint32_t wide = narrow ? sdt : ddt, fp8 = narrow ? ddt : sdt;
+    if (!is_fp8_dtype(fp8) || !(wide == TSNAP_F32 || wide == TSNAP_BF16 || wide == TSNAP_F16)) return 0;
+    if (narrow) {
+        if (wide == TSNAP_F32) cast_fp8_vec_of<true, TSNAP_F32>(fp8, s, d, nelem);
+        else if (wide == TSNAP_BF16) cast_fp8_vec_of<true, TSNAP_BF16>(fp8, s, d, nelem);
+        else cast_fp8_vec_of<true, TSNAP_F16>(fp8, s, d, nelem);
+    } else {
+        if (wide == TSNAP_F32) cast_fp8_vec_of<false, TSNAP_F32>(fp8, s, d, nelem);
+        else if (wide == TSNAP_BF16) cast_fp8_vec_of<false, TSNAP_BF16>(fp8, s, d, nelem);
+        else cast_fp8_vec_of<false, TSNAP_F16>(fp8, s, d, nelem);
+    }
+    return nelem & ~uint64_t(15);
+}
+
 __device__ __noinline__ void tile_cast(const Member& m, uint32_t index) {
     const uint64_t lo = (uint64_t)index * kTileLsu;
     uint64_t hi = lo + kTileLsu;
@@ -760,7 +867,7 @@ __device__ __noinline__ void tile_cast(const Member& m, uint32_t index) {
     const uint64_t e1 = hi / m.dst_esz;
     const char* sb = reinterpret_cast<const char*>(m.src);
     char* db = reinterpret_cast<char*>(m.dst);
-    // fast path: one dense run on both sides, 16 B aligned, fp32 <-> {bf16, fp16}
+    // fast path: one dense run on both sides, 16 B aligned, fp32 <-> {bf16, fp16} or {fp32, bf16, fp16} <-> float8
     if (m.nouter == 0 && ((m.src | m.dst) & 15) == 0) {
         const bool narrow = m.src_dtype == TSNAP_F32 && (m.dst_dtype == TSNAP_BF16 || m.dst_dtype == TSNAP_F16);
         const bool widen = m.dst_dtype == TSNAP_F32 && (m.src_dtype == TSNAP_BF16 || m.src_dtype == TSNAP_F16);
@@ -776,6 +883,9 @@ __device__ __noinline__ void tile_cast(const Member& m, uint32_t index) {
                 else cast_dense_vec<false, false>(s, d, n);
             }
             e0 += n & ~uint64_t(7);  // the ragged tail (< 8 elements) goes through the scalar loop below
+        } else {
+            // {fp32, bf16, fp16} <-> float8; the ragged tail (< 16 elements) goes through the scalar loop below
+            e0 += cast_fp8_dense(m.src_dtype, m.dst_dtype, sb + e0 * m.src_esz, db + e0 * m.dst_esz, e1 - e0);
         }
     }
     if (m.dst_dtype == TSNAP_QINT8 || m.dst_dtype == TSNAP_QUINT8) {

@@ -1,12 +1,14 @@
 #include "plan.h"
 
+#include "fp8.h"
+
 #include <algorithm>
 #include <cmath>
 #include <cstring>
 
 namespace tsnap {
 
-static const size_t kDtypeSize[TSNAP_DTYPE_COUNT] = {1, 1, 2, 4, 8, 2, 2, 4, 8, 1, 1, 1};
+static const size_t kDtypeSize[TSNAP_DTYPE_COUNT] = {1, 1, 2, 4, 8, 2, 2, 4, 8, 1, 1, 1, 1, 1};
 
 size_t dtype_size(int dt) {
     if (dt < 0 || dt >= TSNAP_DTYPE_COUNT) return 0;
@@ -15,11 +17,14 @@ size_t dtype_size(int dt) {
 
 static bool is_float(int dt) { return dt == TSNAP_F16 || dt == TSNAP_BF16 || dt == TSNAP_F32 || dt == TSNAP_F64; }
 
+static bool is_fp8(int dt) { return dt == TSNAP_F8E4M3FN || dt == TSNAP_F8E5M2; }
+
 static bool is_quant(int dt) { return dt == TSNAP_QINT8 || dt == TSNAP_QUINT8; }
 
 bool cast_supported(int s, int d) {
     if (s == d) return !is_quant(s);  // quantised wire elements only exist as the product of a quantising save
-    return is_float(s) && (is_float(d) || is_quant(d));
+    if (is_quant(d)) return is_float(s);  // the quantisers take the four wide floats only
+    return (is_float(s) || is_fp8(s)) && (is_float(d) || is_fp8(d));
 }
 
 // TSNAP_QSCHEME_PER_CHANNEL: float -> quantised on save, and back on restore
@@ -281,6 +286,8 @@ static inline double load_as_double(const void* p, uint32_t dt) {
         case TSNAP_F16: { _Float16 h; std::memcpy(&h, p, 2); return double(float(h)); }
         case TSNAP_BF16: { uint16_t v; std::memcpy(&v, p, 2); return double(bf16_to_f32(v)); }
         case TSNAP_F32: { float f; std::memcpy(&f, p, 4); return double(f); }
+        case TSNAP_F8E4M3FN:
+        case TSNAP_F8E5M2: return double(fp8_to_f32(*static_cast<const uint8_t*>(p), dt));
         default: { double x; std::memcpy(&x, p, 8); return x; }
     }
 }
@@ -294,8 +301,8 @@ static inline uint8_t quantize_host(float x, double scale, int64_t zp, bool is_s
 }
 
 static inline void store_from(void* p, uint32_t dt, const void* sp, uint32_t sdt) {
-    // convert through float when the source is <= 32 bit (exact), through double otherwise; fp64 -> fp16 rounds to fp32
-    // first, as torch does (c10::Half is only built from a float)
+    // convert through float when the source is <= 32 bit (exact), through double otherwise; fp64 -> fp16 and fp64 ->
+    // float8 round to fp32 first, as torch does (c10::Half and c10::Float8_* are only built from a float)
     if (sdt == TSNAP_F64) {
         double x;
         std::memcpy(&x, sp, 8);
@@ -303,6 +310,8 @@ static inline void store_from(void* p, uint32_t dt, const void* sp, uint32_t sdt
             case TSNAP_F16: { _Float16 h = (_Float16)float(x); std::memcpy(p, &h, 2); break; }
             case TSNAP_BF16: { uint16_t v = f32_to_bf16(float(x)); std::memcpy(p, &v, 2); break; }
             case TSNAP_F32: { float f = float(x); std::memcpy(p, &f, 4); break; }
+            case TSNAP_F8E4M3FN:
+            case TSNAP_F8E5M2: *static_cast<uint8_t*>(p) = fp8_from_f32(float(x), dt); break;
             default: std::memcpy(p, &x, 8);
         }
         return;
@@ -312,6 +321,8 @@ static inline void store_from(void* p, uint32_t dt, const void* sp, uint32_t sdt
         case TSNAP_F16: { _Float16 h = (_Float16)f; std::memcpy(p, &h, 2); break; }
         case TSNAP_BF16: { uint16_t v = f32_to_bf16(f); std::memcpy(p, &v, 2); break; }
         case TSNAP_F32: std::memcpy(p, &f, 4); break;
+        case TSNAP_F8E4M3FN:
+        case TSNAP_F8E5M2: *static_cast<uint8_t*>(p) = fp8_from_f32(f, dt); break;
         default: { double x = double(f); std::memcpy(p, &x, 8); }
     }
 }

@@ -23,7 +23,7 @@ from ..manifest import ChunkedTensorEntry, TensorEntry
 from ..native_plan import RAW, describe_consumer, describe_stager, entry_nbytes, raw_castable
 from ..prepare import _FLOATS, PER_CHANNEL_QTENSOR, PER_TENSOR_QTENSOR, PerChannel, fused_quant_of
 from ..serialization import (
-    BUFFER_PROTOCOL_SUPPORTED_DTYPES,
+    RAW_DTYPES,
     SUPPORTED_QUANTIZED_DTYPES,
     Serializer,
     dtype_to_element_size,
@@ -184,7 +184,7 @@ class TensorIOPreparer:
                 "_tensor_prepare_func shouldn't change the tensor's shape "
                 f"(changed from {tensor.shape} to {traced.shape})."
             )
-        serializer = RAW if traced.dtype in BUFFER_PROTOCOL_SUPPORTED_DTYPES else PICKLED
+        serializer = RAW if traced.dtype in RAW_DTYPES else PICKLED
         quant = fused_quant_of(_tensor_prepare_func, tensor) if _tensor_prepare_func is not None else None
         if isinstance(quant, PerChannel):
             serializer = PER_CHANNEL_QTENSOR  # axis header + int_repr + per-channel parameters, produced by the engine

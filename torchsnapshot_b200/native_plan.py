@@ -15,11 +15,11 @@ from typing import Any, List, Optional, Tuple
 import torch
 
 from . import _native
-from .prepare import _FLOATS, PER_CHANNEL_QTENSOR, PER_TENSOR_QTENSOR, PerChannel, fused_cast_of
-from .serialization import BUFFER_PROTOCOL_SUPPORTED_DTYPES, Serializer, dtype_to_element_size, string_to_dtype
+from .prepare import _CASTABLE, _FLOATS, PER_CHANNEL_QTENSOR, PER_TENSOR_QTENSOR, PerChannel, fused_cast_of
+from .serialization import RAW_DTYPES, Serializer, dtype_to_element_size, string_to_dtype
 
 RAW = Serializer.BUFFER_PROTOCOL.value
-_DTYPES = {str(dt): dt for dt in BUFFER_PROTOCOL_SUPPORTED_DTYPES}
+_DTYPES = {str(dt): dt for dt in RAW_DTYPES}
 
 Described = Tuple[List["_native.CopyDesc"], List[torch.Tensor], int]  # descriptors, keep-alive, wire bytes
 
@@ -41,8 +41,8 @@ def entry_nbytes(entry: Any, axis: Optional[int] = None) -> int:
 def raw_castable(src: torch.dtype, dst: torch.dtype) -> bool:
     """dtype pairs the scatter kernel handles itself; others fall back to Tensor.copy_ semantics."""
     if src == dst:
-        return src in BUFFER_PROTOCOL_SUPPORTED_DTYPES
-    return src in _FLOATS and dst in _FLOATS
+        return src in RAW_DTYPES
+    return src in _CASTABLE and dst in _CASTABLE
 
 
 # ---- save side -----------------------------------------------------------------------------------

@@ -13,7 +13,10 @@ from typing import Callable, Optional
 
 import torch
 
-_FLOATS = (torch.float16, torch.bfloat16, torch.float32, torch.float64)
+_FLOATS = (torch.float16, torch.bfloat16, torch.float32, torch.float64)  # what the quantisers (and cast sources) take
+# cast_on_save targets and the float dtypes a restore converts between: the four wide floats and the two plain float8
+# formats (raw 1-byte images, converted with torch's rounding; no scales)
+_CASTABLE = _FLOATS + (torch.float8_e4m3fn, torch.float8_e5m2)
 
 
 class _Traced:
@@ -28,10 +31,14 @@ def cast_on_save(dtype: torch.dtype, only: Optional[str] = None) -> Callable[[st
     """A ``_custom_tensor_prepare_func`` that stores floating-point tensors as ``dtype`` (e.g. fp32 master weights as
     bf16).  ``only``: glob on the logical path; other tensors are stored unchanged.
 
+    ``dtype`` may be ``torch.float8_e4m3fn`` or ``torch.float8_e5m2``: fp64 / fp32 / fp16 / bf16 tensors are then
+    rounded to float8 as ``Tensor.to`` does it (values past e4m3fn's range become NaN, e5m2 overflows to inf).  Tensors
+    that already are float8 are stored unchanged.
+
         Snapshot.take(path, app_state, _custom_tensor_prepare_func=cast_on_save(torch.bfloat16, only="model/*"))
     """
-    if dtype not in _FLOATS:
-        raise ValueError(f"cast_on_save supports {_FLOATS}, not {dtype}")
+    if dtype not in _CASTABLE:
+        raise ValueError(f"cast_on_save supports {_CASTABLE}, not {dtype}")
 
     def applies(logical_path: Optional[str], tensor: torch.Tensor) -> Optional[torch.dtype]:
         if tensor.dtype not in _FLOATS or tensor.dtype == dtype or tensor.is_quantized:

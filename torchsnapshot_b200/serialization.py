@@ -32,6 +32,8 @@ _NAMES: Dict[torch.dtype, str] = {
         torch.qint32,
         torch.qint8,
         torch.quint8,
+        torch.float8_e4m3fn,
+        torch.float8_e5m2,
     )
 }
 _BY_NAME: Dict[str, torch.dtype] = {v: k for k, v in _NAMES.items()}
@@ -40,15 +42,22 @@ _ELEMENT_SIZE: Dict[torch.dtype, int] = {
     torch.complex128: 16, torch.complex64: 8,
     torch.int64: 8, torch.int32: 4, torch.int16: 2, torch.int8: 1, torch.uint8: 1, torch.bool: 1,
     torch.qint32: 4, torch.qint8: 1, torch.quint8: 1,
+    torch.float8_e4m3fn: 1, torch.float8_e5m2: 1,
 }  # fmt: skip
 
-ALL_SUPPORTED_DTYPES: List[torch.dtype] = list(_NAMES)
+# The public lists are exactly the reference's: code written against it (and its own test files) iterates over them
+# and builds test tensors with torch.rand, which has no float8 kernel.  The float8 formats are known to the name and size
+# tables above and travel raw (RAW_DTYPES), but are not listed here.
+FLOAT8_DTYPES: List[torch.dtype] = [torch.float8_e4m3fn, torch.float8_e5m2]
+ALL_SUPPORTED_DTYPES: List[torch.dtype] = [dt for dt in _NAMES if dt not in FLOAT8_DTYPES]
 SUPPORTED_QUANTIZED_DTYPES: List[torch.dtype] = [torch.qint32, torch.qint8, torch.quint8]
 # dtypes whose payload is the raw image (T:serialization.py:162-173); everything else uses torch.save
 BUFFER_PROTOCOL_SUPPORTED_DTYPES: List[torch.dtype] = [
     torch.float64, torch.float32, torch.float16, torch.bfloat16,
     torch.int64, torch.int32, torch.int16, torch.int8, torch.uint8, torch.bool,
 ]  # fmt: skip
+# every dtype whose payload is the raw image: the reference's ten, and the two float8 formats (1-byte images, as int8)
+RAW_DTYPES: List[torch.dtype] = BUFFER_PROTOCOL_SUPPORTED_DTYPES + FLOAT8_DTYPES
 
 
 class Serializer(Enum):
@@ -85,7 +94,7 @@ def dtype_to_element_size(dtype: torch.dtype) -> int:
 
 def tensor_as_memoryview(tensor: torch.Tensor) -> memoryview:
     """Zero-copy raw image of a CPU tensor (a copy is made only if the view is not dense)."""
-    if tensor.dtype not in BUFFER_PROTOCOL_SUPPORTED_DTYPES:
+    if tensor.dtype not in RAW_DTYPES:
         raise ValueError(f"tensor_as_memoryview() doesn't support the dtype {tensor.dtype}.")
     if tensor.device.type != "cpu":
         raise ValueError("tensor_as_memoryview() only accepts CPU tensors.")
