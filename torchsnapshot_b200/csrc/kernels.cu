@@ -17,7 +17,7 @@
 #include <cuda_fp16.h>
 #include <stdint.h>
 
-#include "fp8.h"
+#include "convert.h"
 #include "kernels.h"
 #include "ptx.cuh"
 
@@ -56,12 +56,9 @@ __device__ __forceinline__ bool cursor_next(PieceCursor& c, uint32_t stage_bytes
         if (c.tile >= c.ntiles) return false;
         const Tile t = c.tiles[c.tile];
         const Member* m = c.members + t.member;
-        const uint64_t mbytes = m->bytes;
         c.src = reinterpret_cast<const char*>(m->src);
         c.dst = reinterpret_cast<char*>(m->dst);
-        c.pos = (uint64_t)t.index * kTileBulk;
-        c.end = c.pos + kTileBulk;
-        if (c.end > mbytes) c.end = mbytes;
+        tile_range_bulk(*m, t.index, &c.pos, &c.end);
         c.open = true;
     }
 }
@@ -185,10 +182,7 @@ __device__ __forceinline__ bool rows_next(RowsCursor& c, uint32_t stage_bytes, R
         if (c.tile >= c.ntiles) return false;
         const Tile t = c.tiles[c.tile];
         c.member = t.member;
-        const uint64_t mbytes = c.members[t.member].bytes;
-        c.pos = (uint64_t)t.index * kTileBulk;
-        c.end = c.pos + kTileBulk;
-        if (c.end > mbytes) c.end = mbytes;
+        tile_range_bulk(c.members[t.member], t.index, &c.pos, &c.end);
         c.open = true;
     }
 }
@@ -414,10 +408,8 @@ __device__ __noinline__ void contig_body_shift(const char* s, char* d, uint64_t 
 }
 
 __device__ __forceinline__ void tile_contig(const Member& m, uint32_t index) {
-    const uint64_t a = (uint64_t)index * kTileLsu;
-    uint64_t lo = a > m.shift ? a - m.shift : 0;
-    uint64_t hi = a + kTileLsu - m.shift;
-    if (hi > m.bytes) hi = m.bytes;
+    uint64_t lo, hi;
+    tile_range_contig(m, index, &lo, &hi);
     const char* s = reinterpret_cast<const char*>(m.src) + lo;
     char* d = reinterpret_cast<char*>(m.dst) + lo;
     const uint64_t n = hi - lo;
@@ -435,37 +427,6 @@ __device__ __forceinline__ void tile_contig(const Member& m, uint32_t index) {
     d += head;
     if ((reinterpret_cast<uint64_t>(s) & 15) == 0) contig_body_aligned(s, d, nvec);
     else contig_body_shift(s, d, nvec);
-}
-
-__device__ __forceinline__ void outer_offsets(const Member& m, uint64_t row, int64_t* so, int64_t* dofs) {
-    int64_t s = 0, d = 0;
-    if ((row >> 32) == 0) {
-        uint32_t r = (uint32_t)row;
-        for (int i = (int)m.nouter - 1; i >= 0; --i) {
-            const uint64_t sz64 = (uint64_t)m.osize[i];
-            uint32_t idx;
-            if (sz64 >> 32) {
-                idx = r;
-                r = 0;
-            } else {
-                const uint32_t sz = (uint32_t)sz64;
-                idx = r % sz;
-                r = r / sz;
-            }
-            s += (int64_t)idx * m.sstride[i];
-            d += (int64_t)idx * m.dstride[i];
-        }
-    } else {
-        for (int i = (int)m.nouter - 1; i >= 0; --i) {
-            const uint64_t sz = (uint64_t)m.osize[i];
-            const uint64_t idx = row % sz;
-            row /= sz;
-            s += (int64_t)idx * m.sstride[i];
-            d += (int64_t)idx * m.dstride[i];
-        }
-    }
-    *so = s;
-    *dofs = d;
 }
 
 // row index -> byte offsets on both sides; the single-outer-dim case (2-D narrow / column shard) needs no division
@@ -530,9 +491,8 @@ __device__ __forceinline__ void tile_strided_t(const Member& m, uint64_t lo, uin
 }
 
 __device__ __noinline__ void tile_strided(const Member& m, uint32_t index) {
-    const uint64_t lo = (uint64_t)index * kTileLsu;
-    uint64_t hi = lo + kTileLsu;
-    if (hi > m.bytes) hi = m.bytes;
+    uint64_t lo, hi;
+    tile_range_lsu(m, index, &lo, &hi);
     switch (m.unit) {
         case 16: tile_strided_t<uint4>(m, lo, hi); break;
         case 8: tile_strided_t<uint2>(m, lo, hi); break;
@@ -650,73 +610,6 @@ __device__ __noinline__ void tile_transpose(const Member& m, uint32_t index, uns
 }
 
 // ---- fused cast -------------------------------------------------------------------------------
-__device__ __forceinline__ double load_elem(const char* p, uint32_t dt) {
-    switch (dt) {
-        case TSNAP_F16: return (double)__half2float(*reinterpret_cast<const __half*>(p));
-        case TSNAP_BF16: return (double)__bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(p));
-        case TSNAP_F32: return (double)*reinterpret_cast<const float*>(p);
-        default: return *reinterpret_cast<const double*>(p);
-    }
-}
-__device__ __forceinline__ void store_bytes(char* p, const void* v, int n, bool aligned) {
-    const char* c = reinterpret_cast<const char*>(v);
-    if (aligned) {
-        if (n == 2) *reinterpret_cast<uint16_t*>(p) = *reinterpret_cast<const uint16_t*>(c);
-        else if (n == 4) *reinterpret_cast<uint32_t*>(p) = *reinterpret_cast<const uint32_t*>(c);
-        else *reinterpret_cast<uint64_t*>(p) = *reinterpret_cast<const uint64_t*>(c);
-    } else {
-        for (int i = 0; i < n; ++i) p[i] = c[i];
-    }
-}
-// affine quantisation as torch's CUDA quantize_per_tensor does it: nearbyint(x / scale) + zero_point in double
-// precision, clamped to the integer range (ATen/native/quantized/cuda/AffineQuantizer.cu)
-__device__ __forceinline__ uint8_t quantize_elem(float x, double scale, int64_t zp, bool is_signed) {
-    long long q = (long long)(nearbyint((double)x / scale) + (double)zp);
-    const long long lo = is_signed ? -128 : 0, hi = is_signed ? 127 : 255;
-    q = q < lo ? lo : (q > hi ? hi : q);
-    return (uint8_t)(int8_t)q;
-}
-
-// the n bytes of an element; byte by byte when the source is not element aligned (a wire member behind an odd-sized
-// one in an unpadded slab)
-__device__ __forceinline__ uint64_t load_bits(const char* p, uint32_t n, bool aligned) {
-    if (aligned) return n == 8 ? *reinterpret_cast<const uint64_t*>(p) : n == 4 ? *reinterpret_cast<const uint32_t*>(p) : *reinterpret_cast<const uint16_t*>(p);
-    uint64_t v = 0;
-    for (int i = (int)n - 1; i >= 0; --i) v = (v << 8) | (uint8_t)p[i];
-    return v;
-}
-
-__device__ __forceinline__ void convert_store(char* p, uint32_t ddt, const char* sp, uint32_t sdt, bool src_aligned, bool aligned) {
-    // <=32-bit float sources convert through fp32 (exact widening, with no detour through double: that would quiet the
-    // signalling NaNs torch's bf16 -> fp32 widening keeps bit for bit).  fp64 sources narrow to fp32 and bf16 in one
-    // rounding step, and to fp16 and float8 through fp32: torch's copy kernel has no double -> half or double -> float8
-    // conversion (c10::Half and c10::Float8_* are built from a float), so it rounds twice.  Float8 elements are single
-    // bytes: never misaligned.
-    if (sdt == TSNAP_F64) {
-        const double x = __longlong_as_double((long long)load_bits(sp, 8, src_aligned));
-        if (ddt == TSNAP_F32) { const float f = (float)x; store_bytes(p, &f, 4, aligned); }
-        else if (ddt == TSNAP_F16) { const __half h = __float2half_rn((float)x); store_bytes(p, &h, 2, aligned); }
-        else if (ddt == TSNAP_BF16) { const __nv_bfloat16 b = __float2bfloat16_rn((float)x); store_bytes(p, &b, 2, aligned); }
-        else if (is_fp8_dtype(ddt)) *reinterpret_cast<uint8_t*>(p) = fp8_from_f32((float)x, ddt);
-        else store_bytes(p, &x, 8, aligned);
-        return;
-    }
-    float f;
-    if (is_fp8_dtype(sdt)) {
-        f = fp8_to_f32(*reinterpret_cast<const uint8_t*>(sp), sdt);
-    } else {
-        const uint32_t w = (uint32_t)load_bits(sp, sdt == TSNAP_F32 ? 4 : 2, src_aligned);
-        f = sdt == TSNAP_F32 ? __uint_as_float(w)
-            : sdt == TSNAP_BF16 ? __bfloat162float(__ushort_as_bfloat16((unsigned short)w))
-                                : __half2float(__ushort_as_half((unsigned short)w));
-    }
-    if (ddt == TSNAP_F32) store_bytes(p, &f, 4, aligned);
-    else if (ddt == TSNAP_F16) { const __half h = __float2half_rn(f); store_bytes(p, &h, 2, aligned); }
-    else if (ddt == TSNAP_BF16) { const __nv_bfloat16 b = __float2bfloat16_rn(f); store_bytes(p, &b, 2, aligned); }
-    else if (is_fp8_dtype(ddt)) *reinterpret_cast<uint8_t*>(p) = fp8_from_f32(f, ddt);
-    else { const double x = (double)f; store_bytes(p, &x, 8, aligned); }
-}
-
 // dense, 16 B aligned, 2-byte <-> 4-byte float conversions: 8 elements per thread, 16 B accesses
 template <bool kNarrow, bool kBf16>
 __device__ __forceinline__ void cast_dense_vec(const char* __restrict__ s, char* __restrict__ d, uint64_t nelem) {
@@ -860,9 +753,8 @@ __device__ __forceinline__ uint64_t cast_fp8_dense(uint32_t sdt, uint32_t ddt, c
 }
 
 __device__ __noinline__ void tile_cast(const Member& m, uint32_t index) {
-    const uint64_t lo = (uint64_t)index * kTileLsu;
-    uint64_t hi = lo + kTileLsu;
-    if (hi > m.bytes) hi = m.bytes;
+    uint64_t lo, hi;
+    tile_range_lsu(m, index, &lo, &hi);
     uint64_t e0 = lo / m.dst_esz;
     const uint64_t e1 = hi / m.dst_esz;
     const char* sb = reinterpret_cast<const char*>(m.src);
@@ -895,7 +787,7 @@ __device__ __noinline__ void tile_cast(const Member& m, uint32_t index) {
             const uint64_t row = e / m.inner, col = e - row * m.inner;
             int64_t so, dofs;
             outer_offsets(m, row, &so, &dofs);
-            const float x = (float)load_elem(sb + so + col * m.src_esz, m.src_dtype);
+            const float x = load_f32(sb + so + col * m.src_esz, m.src_dtype, true);
             reinterpret_cast<uint8_t*>(db + dofs)[col] = quantize_elem(x, m.q_scale, m.q_zero_point, is_signed);
         }
         if ((m.shift & 1) && hi == m.bytes && threadIdx.x < 16) {
@@ -950,11 +842,10 @@ __global__ void __launch_bounds__(kLsuThreads, kMinBlocks) tsnap_lsu_copy_kernel
             default: {
                 // unreachable: kernel_of sends every other mode to another kernel.  Kept for robustness: a
                 // bulk-mode member, dense and 16B aligned on both sides
-                const uint64_t a = (uint64_t)tl.index * kTileLsu;
-                uint64_t hi = a + kTileLsu;
-                if (hi > sm.bytes) hi = sm.bytes;
-                contig_body_aligned(reinterpret_cast<const char*>(sm.src) + a, reinterpret_cast<char*>(sm.dst) + a,
-                                    (hi - a) >> 4);
+                uint64_t lo, hi;
+                tile_range_lsu(sm, tl.index, &lo, &hi);
+                contig_body_aligned(reinterpret_cast<const char*>(sm.src) + lo, reinterpret_cast<char*>(sm.dst) + lo,
+                                    (hi - lo) >> 4);
             }
         }
     }
@@ -1018,10 +909,6 @@ __device__ __forceinline__ void st_u64_any(char* p, uint64_t v) {
     for (int i = 0; i < 8; ++i) p[i] = (char)(v >> (8 * i));
 }
 
-__device__ __forceinline__ void st_bytes_any(char* p, uint32_t v, int n) {
-    for (int i = 0; i < n; ++i) p[i] = (char)(v >> (8 * i));
-}
-
 // The source elements of save chunk [e, e + n) as fp32 (the value the quantiser reads); 16 B loads when the chunk is
 // a full, 16 B-aligned piece of one dense run.
 __device__ __forceinline__ void qload_chunk(const Member& m, uint64_t e, uint32_t n, float (&x)[kQChunk]) {
@@ -1058,7 +945,7 @@ __device__ __forceinline__ void qload_chunk(const Member& m, uint64_t e, uint32_
 #pragma unroll
     for (uint32_t i = 0; i < kQChunk; ++i) {
         if (i < n) {
-            x[i] = (float)load_elem(sb + w.so + w.col * m.src_esz, m.src_dtype);
+            x[i] = load_f32(sb + w.so + w.col * m.src_esz, m.src_dtype, true);
             qwalk_next(m, w);
         }
     }
@@ -1099,7 +986,8 @@ __global__ void __launch_bounds__(kLsuThreads) tsnap_qstats_kernel(const Member*
         const Tile tl = tiles[t];
         const Member& m = members[tl.member];
         const QChannel q = qch[m.q_zero_point];
-        const uint64_t lo = (uint64_t)tl.index * kTileLsu, hi = lo + kTileLsu < m.bytes ? lo + kTileLsu : m.bytes;
+        uint64_t lo, hi;
+        tile_range_lsu(m, tl.index, &lo, &hi);
         const bool shared = q.channels <= kQSmemChannels;
         int* keys = reinterpret_cast<int*>(q.keys);
         __syncthreads();  // the table is clean
@@ -1218,7 +1106,8 @@ __global__ void __launch_bounds__(kLsuThreads) tsnap_qchannel_kernel(const Membe
         const Tile tl = tiles[t];
         const Member& m = members[tl.member];
         const QChannel q = qch[m.q_zero_point];
-        const uint64_t lo = (uint64_t)tl.index * kTileLsu, hi = lo + kTileLsu < m.bytes ? lo + kTileLsu : m.bytes;
+        uint64_t lo, hi;
+        tile_range_lsu(m, tl.index, &lo, &hi);
         if (q.save) {
             const bool is_signed = m.dst_dtype == TSNAP_QINT8;
             const uint2* kp = reinterpret_cast<const uint2*>(q.keys);                       // (1 / scale: f32, zero_point: i32)
@@ -1302,8 +1191,7 @@ __global__ void __launch_bounds__(kLsuThreads) tsnap_qchannel_kernel(const Membe
                 } else {
                     uint16_t h[4];
 #pragma unroll
-                    for (int i = 0; i < 4; ++i)
-                        h[i] = m.dst_dtype == TSNAP_BF16 ? __bfloat16_as_ushort(__float2bfloat16_rn(f[i])) : __half_as_ushort(__float2half_rn(f[i]));
+                    for (int i = 0; i < 4; ++i) h[i] = f16_or_bf16_from_f32(f[i], m.dst_dtype);
                     *reinterpret_cast<uint2*>(p) = make_uint2(h[0] | ((uint32_t)h[1] << 16), h[2] | ((uint32_t)h[3] << 16));
                 }
             }
@@ -1311,12 +1199,9 @@ __global__ void __launch_bounds__(kLsuThreads) tsnap_qchannel_kernel(const Membe
                 for (uint64_t e = e0 + 4 * ngroups; e < e1; ++e) {
                     uint64_t c, r;
                     qchan_at(q, m.src + e, &c, &r);
-                    const uint8_t raw = (uint8_t)sb[e];
-                    const int64_t v = is_signed ? (int64_t)(int8_t)raw : (int64_t)raw;
-                    const float f = (float)((double)(v - (int64_t)ld_u64_any(params + 8 * (q.channels + c))) * __longlong_as_double((long long)ld_u64_any(params + 8 * c)));
-                    char* p = db + e * m.dst_esz;
-                    if (m.dst_dtype == TSNAP_F32) *reinterpret_cast<float*>(p) = f;
-                    else *reinterpret_cast<uint16_t*>(p) = m.dst_dtype == TSNAP_BF16 ? __bfloat16_as_ushort(__float2bfloat16_rn(f)) : __half_as_ushort(__float2half_rn(f));
+                    const float f = dequantize((uint8_t)sb[e], is_signed, (int64_t)ld_u64_any(params + 8 * (q.channels + c)),
+                                               __longlong_as_double((long long)ld_u64_any(params + 8 * c)));
+                    store_f32(db + e * m.dst_esz, m.dst_dtype, f, true);
                 }
             }
             continue;
@@ -1328,22 +1213,9 @@ __global__ void __launch_bounds__(kLsuThreads) tsnap_qchannel_kernel(const Membe
             uint64_t c, r;
             qchan_at(q, m.src + w.so + w.col, &c, &r);
             for (uint32_t i = 0; i < n; ++i) {
-                const uint8_t raw = (uint8_t)sb[w.so + w.col];
-                const int64_t v = is_signed ? (int64_t)(int8_t)raw : (int64_t)raw;
                 const double scale = __longlong_as_double((long long)ld_u64_any(params + 8 * c));
                 const int64_t zp = (int64_t)ld_u64_any(params + 8 * (q.channels + c));
-                const float f = (float)((double)(v - zp) * scale);
-                char* p = db + w.dofs + w.col * m.dst_esz;
-                if (m.dst_dtype == TSNAP_F32) {
-                    if (aligned) *reinterpret_cast<float*>(p) = f;
-                    else st_bytes_any(p, __float_as_uint(f), 4);
-                } else if (m.dst_dtype == TSNAP_F64) {
-                    st_u64_any(p, (uint64_t)__double_as_longlong((double)f));
-                } else {
-                    const uint16_t h = m.dst_dtype == TSNAP_BF16 ? __bfloat16_as_ushort(__float2bfloat16_rn(f)) : __half_as_ushort(__float2half_rn(f));
-                    if (aligned) *reinterpret_cast<uint16_t*>(p) = h;
-                    else st_bytes_any(p, h, 2);
-                }
+                store_f32(db + w.dofs + w.col * m.dst_esz, m.dst_dtype, dequantize((uint8_t)sb[w.so + w.col], is_signed, zp, scale), aligned);
                 if (qwalk_next(m, w)) qchan_at(q, m.src + w.so, &c, &r);
                 else qchan_next(q, &c, &r);
             }

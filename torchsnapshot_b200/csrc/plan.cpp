@@ -1,7 +1,5 @@
 #include "plan.h"
 
-#include "fp8.h"
-
 #include <algorithm>
 #include <cmath>
 #include <cstring>
@@ -17,14 +15,12 @@ size_t dtype_size(int dt) {
 
 static bool is_float(int dt) { return dt == TSNAP_F16 || dt == TSNAP_BF16 || dt == TSNAP_F32 || dt == TSNAP_F64; }
 
-static bool is_fp8(int dt) { return dt == TSNAP_F8E4M3FN || dt == TSNAP_F8E5M2; }
-
 static bool is_quant(int dt) { return dt == TSNAP_QINT8 || dt == TSNAP_QUINT8; }
 
 bool cast_supported(int s, int d) {
     if (s == d) return !is_quant(s);  // quantised wire elements only exist as the product of a quantising save
     if (is_quant(d)) return is_float(s);  // the quantisers take the four wide floats only
-    return (is_float(s) || is_fp8(s)) && (is_float(d) || is_fp8(d));
+    return (is_float(s) || is_fp8_dtype(s)) && (is_float(d) || is_fp8_dtype(d));
 }
 
 // TSNAP_QSCHEME_PER_CHANNEL: float -> quantised on save, and back on restore
@@ -265,81 +261,6 @@ int normalize_copy(const tsnap_copy_desc& d, uint64_t wire_base, bool allow_bulk
 
 // ---- host execution -------------------------------------------------------------------------------------
 
-static inline float bf16_to_f32(uint16_t v) {
-    uint32_t u = uint32_t(v) << 16;
-    float f;
-    std::memcpy(&f, &u, 4);
-    return f;
-}
-// round-to-nearest-even (c10::BFloat16's rounding), NaN -> 0x7FC0.  torch's CPU path has no fixed NaN encoding: fp32 ->
-// bf16 writes 0xFFFF, fp64 -> bf16 0x7FC0 or 0xFFFF depending on whether its scalar or vectorised loop ran.
-static inline uint16_t f32_to_bf16(float f) {
-    if (std::isnan(f)) return 0x7FC0;
-    uint32_t u;
-    std::memcpy(&u, &f, 4);
-    uint32_t bias = ((u >> 16) & 1) + 0x7FFFu;
-    return uint16_t((u + bias) >> 16);
-}
-
-static inline double load_as_double(const void* p, uint32_t dt) {
-    switch (dt) {
-        case TSNAP_F16: { _Float16 h; std::memcpy(&h, p, 2); return double(float(h)); }
-        case TSNAP_BF16: { uint16_t v; std::memcpy(&v, p, 2); return double(bf16_to_f32(v)); }
-        case TSNAP_F32: { float f; std::memcpy(&f, p, 4); return double(f); }
-        case TSNAP_F8E4M3FN:
-        case TSNAP_F8E5M2: return double(fp8_to_f32(*static_cast<const uint8_t*>(p), dt));
-        default: { double x; std::memcpy(&x, p, 8); return x; }
-    }
-}
-// torch's CPU quantize_val (non-FBGEMM build, c10::qint8/quint8): zero_point + nearbyint(value * (1.0f / scale))
-static inline uint8_t quantize_host(float x, double scale, int64_t zp, bool is_signed) {
-    const float inv = 1.0f / float(scale);
-    int64_t q = zp + int64_t(std::nearbyint(x * inv));
-    const int64_t lo = is_signed ? -128 : 0, hi = is_signed ? 127 : 255;
-    q = q < lo ? lo : (q > hi ? hi : q);
-    return uint8_t(int8_t(q));
-}
-
-static inline void store_from(void* p, uint32_t dt, const void* sp, uint32_t sdt) {
-    // convert through float when the source is <= 32 bit (exact), through double otherwise; fp64 -> fp16 and fp64 ->
-    // float8 round to fp32 first, as torch does (c10::Half and c10::Float8_* are only built from a float)
-    if (sdt == TSNAP_F64) {
-        double x;
-        std::memcpy(&x, sp, 8);
-        switch (dt) {
-            case TSNAP_F16: { _Float16 h = (_Float16)float(x); std::memcpy(p, &h, 2); break; }
-            case TSNAP_BF16: { uint16_t v = f32_to_bf16(float(x)); std::memcpy(p, &v, 2); break; }
-            case TSNAP_F32: { float f = float(x); std::memcpy(p, &f, 4); break; }
-            case TSNAP_F8E4M3FN:
-            case TSNAP_F8E5M2: *static_cast<uint8_t*>(p) = fp8_from_f32(float(x), dt); break;
-            default: std::memcpy(p, &x, 8);
-        }
-        return;
-    }
-    float f = float(load_as_double(sp, sdt));
-    switch (dt) {
-        case TSNAP_F16: { _Float16 h = (_Float16)f; std::memcpy(p, &h, 2); break; }
-        case TSNAP_BF16: { uint16_t v = f32_to_bf16(f); std::memcpy(p, &v, 2); break; }
-        case TSNAP_F32: std::memcpy(p, &f, 4); break;
-        case TSNAP_F8E4M3FN:
-        case TSNAP_F8E5M2: *static_cast<uint8_t*>(p) = fp8_from_f32(f, dt); break;
-        default: { double x = double(f); std::memcpy(p, &x, 8); }
-    }
-}
-
-static inline void outer_offsets(const Member& m, uint64_t row, int64_t* so, int64_t* dofs) {
-    int64_t s = 0, d = 0;
-    for (int i = int(m.nouter) - 1; i >= 0; --i) {
-        const uint64_t sz = uint64_t(m.osize[i]);
-        const uint64_t idx = row % sz;
-        row /= sz;
-        s += int64_t(idx) * m.sstride[i];
-        d += int64_t(idx) * m.dstride[i];
-    }
-    *so = s;
-    *dofs = d;
-}
-
 void host_copy_range(const Member& m, uint64_t lo, uint64_t hi) {
     if (hi > m.bytes) hi = m.bytes;
     if (lo >= hi) return;
@@ -362,7 +283,8 @@ void host_copy_range(const Member& m, uint64_t lo, uint64_t hi) {
         }
         return;
     }
-    // cast: lo/hi are dst bytes, multiples of the dst element size by construction
+    // cast: lo/hi are dst bytes, multiples of the dst element size by construction.  Elements are read and written
+    // byte by byte (aligned = false): host pointers may sit at any alignment, and the compiler merges the bytes.
     const uint64_t e0 = lo / m.dst_esz, e1 = hi / m.dst_esz;
     const bool quant = m.dst_dtype == TSNAP_QINT8 || m.dst_dtype == TSNAP_QUINT8;
     for (uint64_t e = e0; e < e1; ++e) {
@@ -370,10 +292,10 @@ void host_copy_range(const Member& m, uint64_t lo, uint64_t hi) {
         int64_t so, dofs;
         outer_offsets(m, row, &so, &dofs);
         if (quant) {
-            const float x = float(load_as_double(src + so + col * m.src_esz, m.src_dtype));
-            reinterpret_cast<uint8_t*>(dst + dofs)[col] = quantize_host(x, m.q_scale, m.q_zero_point, m.dst_dtype == TSNAP_QINT8);
+            const float x = load_f32(src + so + col * m.src_esz, m.src_dtype, false);
+            reinterpret_cast<uint8_t*>(dst + dofs)[col] = quantize_elem(x, m.q_scale, m.q_zero_point, m.dst_dtype == TSNAP_QINT8);
         } else {
-            store_from(dst + dofs + col * m.dst_esz, m.dst_dtype, src + so + col * m.src_esz, m.src_dtype);
+            convert_store(dst + dofs + col * m.dst_esz, m.dst_dtype, src + so + col * m.src_esz, m.src_dtype, false, false);
         }
     }
     if (quant && (m.shift & 1) && hi == m.bytes) {
@@ -383,15 +305,6 @@ void host_copy_range(const Member& m, uint64_t lo, uint64_t hi) {
 }
 
 // ---- per-channel quantisation on the host ------------------------------------------------------------------
-static inline void store_float(void* p, uint32_t dt, float f) {
-    switch (dt) {
-        case TSNAP_F16: { _Float16 h = (_Float16)f; std::memcpy(p, &h, 2); break; }
-        case TSNAP_BF16: { uint16_t v = f32_to_bf16(f); std::memcpy(p, &v, 2); break; }
-        case TSNAP_F32: std::memcpy(p, &f, 4); break;
-        default: { double x = double(f); std::memcpy(p, &x, 8); }
-    }
-}
-
 // The three passes of the device (statistics, parameters, quantising pack) in one sequential sweep each, with the same
 // rules: the element as fp32, channel keys that start at 0, the parameters of qparams_of, torch's CPU quantiser.
 int host_qchannel(const Member& m, const QChannel& q, std::string* err) {
@@ -413,8 +326,7 @@ int host_qchannel(const Member& m, const QChannel& q, std::string* err) {
             std::memcpy(&scale, params + 8 * c, 8);
             std::memcpy(&zp, params + 8 * (q.channels + c), 8);
             const uint8_t raw = *reinterpret_cast<const uint8_t*>(uintptr_t(a));
-            const int64_t v = is_signed ? int64_t(int8_t(raw)) : int64_t(raw);
-            store_float(dst + dofs + col * m.dst_esz, m.dst_dtype, float(double(v - zp) * scale));
+            store_f32(dst + dofs + col * m.dst_esz, m.dst_dtype, dequantize(raw, is_signed, zp, scale), false);
         }
         return TSNAP_OK;
     }
@@ -423,7 +335,7 @@ int host_qchannel(const Member& m, const QChannel& q, std::string* err) {
         const uint64_t row = e / m.inner, col = e % m.inner;
         int64_t so, dofs;
         outer_offsets(m, row, &so, &dofs);
-        const int32_t k = qkey(float(load_as_double(src + so + col * m.src_esz, m.src_dtype)));
+        const int32_t k = qkey(load_f32(src + so + col * m.src_esz, m.src_dtype, false));
         const uint64_t c = channel(m.dst + uint64_t(dofs) + col);
         kmin[c] = std::min(kmin[c], k);
         kmax[c] = std::max(kmax[c], k);
@@ -443,9 +355,9 @@ int host_qchannel(const Member& m, const QChannel& q, std::string* err) {
         const uint64_t row = e / m.inner, col = e % m.inner;
         int64_t so, dofs;
         outer_offsets(m, row, &so, &dofs);
-        const float x = float(load_as_double(src + so + col * m.src_esz, m.src_dtype));
+        const float x = load_f32(src + so + col * m.src_esz, m.src_dtype, false);
         const uint64_t c = channel(m.dst + uint64_t(dofs) + col);
-        reinterpret_cast<uint8_t*>(dst + dofs)[col] = quantize_host(x, scale[c], zp[c], is_signed);
+        reinterpret_cast<uint8_t*>(dst + dofs)[col] = quantize_elem(x, scale[c], zp[c], is_signed);
     }
     return TSNAP_OK;
 }

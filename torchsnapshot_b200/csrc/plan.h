@@ -1,6 +1,6 @@
 // Planner: turns tsnap_copy_desc (strided view <-> strided view, torch-style element strides) into
 // normalised members and a tile cover.  Shared by the device kernels (kernels.cu) and the host
-// executor (host_exec.cpp), so the CPU test-suite exercises the same decomposition the GPU runs.
+// executor (plan.cpp), so the CPU test-suite exercises the same decomposition the GPU runs.
 //
 // What is being restated here: the reference makes every source "contiguous" first
 // (T:batcher.py:156 `tensor.contiguous()`, T:serialization.py:196 `tensor.contiguous()`) and then does
@@ -13,16 +13,11 @@
 #include <string>
 #include <vector>
 
-#include "../../include/tsnap_b200.h"
+#include "convert.h"
 
 namespace tsnap {
 
 constexpr int kMaxOuter = 8;
-#ifdef __CUDACC__
-#define TSNAP_HD __host__ __device__
-#else
-#define TSNAP_HD
-#endif
 constexpr uint32_t kTileBulk = 192 * 1024;  // bytes of one bulk (TMA) tile: a multiple of every ring stage size
 constexpr uint32_t kTileLsu = 128 * 1024;  // logical dst bytes of one LSU tile (per-tile setup costs ~2 dependent global round trips)
 constexpr uint64_t kBulkMin = 1024;        // contiguous runs shorter than this stay on the LSU path
@@ -102,20 +97,20 @@ constexpr int kTmaMaxOther = 3;                // dims besides A and B a rank-5 
 // and <= 256 elements (TMA box limit).  Variant (Member.shift bits 16-17): 0 square-ish, 1 twice as long along A,
 // 2 twice as long along B — the engine picks the one that pads the member's two extents least.
 constexpr uint32_t kTmaVariantShift = 16, kTmaVariants = 3;
-TSNAP_HD inline uint32_t transpose_tma_side_a(uint32_t esz, uint32_t variant) {
+TSNAP_HD uint32_t transpose_tma_side_a(uint32_t esz, uint32_t variant) {
     const uint32_t a = esz == 2 ? 128 : 64;
     return variant == 1 ? a * 2 : variant == 2 ? a / 2 : a;
 }
-TSNAP_HD inline uint32_t transpose_tma_side_b(uint32_t esz, uint32_t variant) {
+TSNAP_HD uint32_t transpose_tma_side_b(uint32_t esz, uint32_t variant) {
     const uint32_t b = esz == 8 ? 64 : 128;
     return variant == 1 ? b / 2 : variant == 2 ? b * 2 : b;
 }
-TSNAP_HD inline uint32_t transpose_tma_variant_of(uint32_t shift) { return (shift >> kTmaVariantShift) & 3; }
+TSNAP_HD uint32_t transpose_tma_variant_of(uint32_t shift) { return (shift >> kTmaVariantShift) & 3; }
 // kModeRowsTma: tensor maps over 8-byte elements, dims {run / 8, last outer dim, the other outer dims from the last down};
 // one tile = one box of `rows` consecutive runs along the last outer dim, at most kTmaTileBytes
 constexpr uint64_t kRowsTmaMaxRun = 1024;  // longer runs amortise one copy-engine request per run (the rows kernel)
 constexpr int kRowsTmaMaxOuter = 4;
-TSNAP_HD inline uint32_t rows_tma_box_rows(uint64_t run) {
+TSNAP_HD uint32_t rows_tma_box_rows(uint64_t run) {
     const uint64_t r = kTmaTileBytes / run;
     return uint32_t(r > 256 ? 256 : r);
 }
@@ -125,16 +120,15 @@ struct Tile {
     uint32_t index;   // tile ordinal within the member
 };
 
-inline bool engine_mode(uint32_t mode) { return mode == kModeBulk || mode == kModeRows; }  // copy-engine kernels
-inline uint32_t tile_bytes_for(uint32_t mode) { return engine_mode(mode) ? kTileBulk : kTileLsu; }
+TSNAP_HD bool engine_mode(uint32_t mode) { return mode == kModeBulk || mode == kModeRows; }  // copy-engine kernels
 
 // kModeTranspose: elements per tile along A (the source-contiguous dim) and B (the destination-contiguous dim):
 // 16 KiB of payload per tile (4 x 16 B vectors per thread), small enough for 6 resident CTAs per SM
-inline uint32_t transpose_side_a(uint32_t esz) { return esz >= 4 ? 64 : 128; }
-inline uint32_t transpose_side_b(uint32_t esz) { return esz == 8 ? 32 : esz == 1 ? 128 : 64; }
+TSNAP_HD uint32_t transpose_side_a(uint32_t esz) { return esz >= 4 ? 64 : 128; }
+TSNAP_HD uint32_t transpose_side_b(uint32_t esz) { return esz == 8 ? 32 : esz == 1 ? 128 : 64; }
 
 // number of tiles a member needs
-inline uint64_t tile_count(const Member& m) {
+TSNAP_HD uint64_t tile_count(const Member& m) {
     if (m.bytes == 0) return 0;
     if (m.mode == kModeTranspose || m.mode == kModeTransposeTma) {
         const bool tma = m.mode == kModeTransposeTma;
@@ -157,20 +151,63 @@ inline uint64_t tile_count(const Member& m) {
     return (m.bytes + kTileLsu - 1) / kTileLsu;
 }
 
-// logical byte range [lo, hi) of tile `index` of member m  (host+device identical: see kernels.cu)
-inline void tile_range(const Member& m, uint32_t index, uint64_t* lo, uint64_t* hi) {
-    if (engine_mode(m.mode)) {
-        *lo = uint64_t(index) * kTileBulk;
-        *hi = *lo + kTileBulk;
-    } else if (m.mode == kModeContig) {
-        uint64_t a = uint64_t(index) * kTileLsu;
-        *lo = a > m.shift ? a - m.shift : 0;
-        *hi = a + kTileLsu - m.shift;
-    } else {
-        *lo = uint64_t(index) * kTileLsu;
-        *hi = *lo + kTileLsu;
-    }
+// Logical byte range [lo, hi) of tile `index` of member m, the range the kernels copy.  One helper per tile family: a
+// kernel knows its family and calls that one, tile_range picks it by mode.  (Transpose and kModeRowsTma tiles are
+// blocks of elements or runs instead.)
+TSNAP_HD void tile_range_bulk(const Member& m, uint32_t index, uint64_t* lo, uint64_t* hi) {  // kModeBulk, kModeRows
+    const uint64_t bytes = m.bytes;
+    *lo = uint64_t(index) * kTileBulk;
+    *hi = *lo + kTileBulk < bytes ? *lo + kTileBulk : bytes;
+}
+// kModeContig: tile boundaries sit on 16 B boundaries of the destination, so the first tile is m.shift bytes short
+TSNAP_HD void tile_range_contig(const Member& m, uint32_t index, uint64_t* lo, uint64_t* hi) {
+    const uint64_t a = uint64_t(index) * kTileLsu;
+    *lo = a > m.shift ? a - m.shift : 0;
+    *hi = a + kTileLsu - m.shift;
     if (*hi > m.bytes) *hi = m.bytes;
+}
+// the other LSU modes, and the per-channel statistics and quantising or dequantising passes
+TSNAP_HD void tile_range_lsu(const Member& m, uint32_t index, uint64_t* lo, uint64_t* hi) {
+    *lo = uint64_t(index) * kTileLsu;
+    *hi = *lo + kTileLsu;
+    if (*hi > m.bytes) *hi = m.bytes;
+}
+TSNAP_HD void tile_range(const Member& m, uint32_t index, uint64_t* lo, uint64_t* hi) {
+    if (engine_mode(m.mode)) tile_range_bulk(m, index, lo, hi);
+    else if (m.mode == kModeContig) tile_range_contig(m, index, lo, hi);
+    else tile_range_lsu(m, index, lo, hi);
+}
+
+// row index -> byte offsets of the row on both sides; 32-bit division while the row index fits
+TSNAP_HD void outer_offsets(const Member& m, uint64_t row, int64_t* so, int64_t* dofs) {
+    int64_t s = 0, d = 0;
+    if ((row >> 32) == 0) {
+        uint32_t r = (uint32_t)row;
+        for (int i = (int)m.nouter - 1; i >= 0; --i) {
+            const uint64_t sz64 = (uint64_t)m.osize[i];
+            uint32_t idx;
+            if (sz64 >> 32) {
+                idx = r;
+                r = 0;
+            } else {
+                const uint32_t sz = (uint32_t)sz64;
+                idx = r % sz;
+                r = r / sz;
+            }
+            s += (int64_t)idx * m.sstride[i];
+            d += (int64_t)idx * m.dstride[i];
+        }
+    } else {
+        for (int i = (int)m.nouter - 1; i >= 0; --i) {
+            const uint64_t sz = (uint64_t)m.osize[i];
+            const uint64_t idx = row % sz;
+            row /= sz;
+            s += (int64_t)idx * m.sstride[i];
+            d += (int64_t)idx * m.dstride[i];
+        }
+    }
+    *so = s;
+    *dofs = d;
 }
 
 struct NormalizedCopy {
@@ -202,29 +239,15 @@ int host_copy_all(const NormalizedCopy& nc, std::string* err);
 // Ordered-int key of a float (signed comparison of keys == float comparison for non-NaN values), and back.  The
 // statistics pass keeps the running min / max of a channel as two keys; both start at key(0.0f) = 0, so every range
 // includes 0 — exactly what both default rules need.
-TSNAP_HD inline int32_t qkey(float f) {
-    int32_t i;
-#ifdef __CUDA_ARCH__
-    i = __float_as_int(f);
-#else
-    __builtin_memcpy(&i, &f, 4);
-#endif
+TSNAP_HD int32_t qkey(float f) {
+    const int32_t i = (int32_t)f32_bits(f);
     return i >= 0 ? i : i ^ 0x7fffffff;
 }
-TSNAP_HD inline float qkey_value(int32_t k) {
-    const int32_t i = k >= 0 ? k : k ^ 0x7fffffff;
-    float f;
-#ifdef __CUDA_ARCH__
-    f = __int_as_float(i);
-#else
-    __builtin_memcpy(&f, &i, 4);
-#endif
-    return f;
-}
+TSNAP_HD float qkey_value(int32_t k) { return f32_from_bits(uint32_t(k >= 0 ? k : k ^ 0x7fffffff)); }
 constexpr int32_t kQKeyMax = 0x7f7fffff;                  // key of FLT_MAX: larger keys are +Inf / NaN
 constexpr int32_t kQKeyMin = int32_t(0xff7fffffu ^ 0x7fffffffu);  // key of -FLT_MAX: smaller keys are -Inf / NaN
 // (scale, zero_point) of one channel from its (min, max) keys, in double as the default rule states; false on NaN / Inf
-TSNAP_HD inline bool qparams_of(int32_t kmin, int32_t kmax, bool is_signed, double* scale, int64_t* zp) {
+TSNAP_HD bool qparams_of(int32_t kmin, int32_t kmax, bool is_signed, double* scale, int64_t* zp) {
     if (kmax > kQKeyMax || kmin < kQKeyMin) return false;
     const double lo = (double)qkey_value(kmin), hi = (double)qkey_value(kmax);
     if (is_signed) {
