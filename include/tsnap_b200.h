@@ -114,14 +114,23 @@ typedef struct tsnap_copy_desc {
  *              and writes the axis header, the int body and both parameter arrays.  A NaN or Inf fails the call / job.
  *     restore: src_dtype QINT8 / QUINT8 in WIRE (the piece or a sub-box of it), dst = float view of any float dtype:
  *              float((q - zero_point) * scale) converted to the destination dtype.
+ *   PER_CHANNEL with a float8 wire dtype (F8E4M3FN / F8E5M2): this library's scaled float8 format
+ *       [axis: int64][float8 bytes, C order][scales: float32 x C]
+ *     save   : src = F16 / BF16 / F32 / F64 view, dst_dtype F8E4M3FN / F8E5M2 in WIRE at body_addr.  With x the element
+ *              as fp32 (fp64 rounds once) and FMAX 448 (e4m3fn) or 57344 (e5m2): s = amax(|x|) / FMAX in IEEE fp32
+ *              division, 1 when that is 0; q = float8(clamp(x / s, -FMAX, FMAX)), again an IEEE division, then torch's
+ *              rounding.  Writes the axis header, the float8 body and the scales.  A NaN or Inf fails the call / job.
+ *     restore: float8 WIRE (piece or sub-box) -> float view of F16 / BF16 / F32 / F64: fp32(q) * s in fp32, then
+ *              converted once to the destination dtype.
+ *     Every other pair under PER_CHANNEL (float8 <-> float8, float8 <-> int, ...) is TSNAP_EUNSUP.
  *   The channel of wire element e is ((e - body_addr) / inner) % channels. */
 #define TSNAP_QSCHEME_PER_TENSOR 0
 #define TSNAP_QSCHEME_PER_CHANNEL 1
 typedef struct tsnap_qchannel {
     int64_t channels;     /* C = piece shape[axis]                                            */
     int64_t inner;        /* prod(piece shape after axis)                                     */
-    uint64_t body_addr;   /* WIRE offset of the piece's first int element (the header is 8 B before it) */
-    uint64_t params_addr; /* WIRE offset of scales[C]; zero_points[C] follow                  */
+    uint64_t body_addr;   /* WIRE offset of the piece's first int / float8 element (the header is 8 B before it) */
+    uint64_t params_addr; /* WIRE offset of scales[C] (f64, zero_points[C] follow; f32 for float8) = body_addr + numel */
     int64_t axis;         /* written into the header on save                                  */
 } tsnap_qchannel;
 

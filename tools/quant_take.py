@@ -1,8 +1,8 @@
-"""Per-channel int8 quantise-on-save and the e4m3fn cast on the C3 checkpoint (FSDP-layout Llama-3-8B bf16, one rank:
-291 tensors, 16.06 GB).
+"""Per-channel int8 quantise-on-save, per-channel scaled float8 and the e4m3fn cast on the C3 checkpoint (FSDP-layout
+Llama-3-8B bf16, one rank: 291 tensors, 16.06 GB).
 
-For each of two alternating rounds, and for the plain snapshot, ``quantize_on_save(torch.qint8, axis=0)`` and
-``cast_on_save(torch.float8_e4m3fn)``:
+For each of two alternating rounds, and for the plain snapshot, ``quantize_on_save(torch.qint8, axis=0)``,
+``quantize_on_save(torch.float8_e4m3fn, axis=0)`` and ``cast_on_save(torch.float8_e4m3fn)``:
 ``Snapshot.take`` and ``restore`` wall time, bytes on disk, and how long ``async_take`` blocks the caller.  The card's
 name and power limit are read in the same run.  Prints one JSON line per (round, variant) and a summary line.
 
@@ -66,7 +66,8 @@ def main() -> None:
         app = {"model": B.StateDict(**W.wrap_sharded(local, 0, dev))}
         payload = sum(t.numel() * t.element_size() for t, _, _ in local.values())
         info = card()
-        hooks = {"plain": None, "qint8_axis0": B.quantize_on_save(torch.qint8, axis=0), "e4m3fn_cast": B.cast_on_save(torch.float8_e4m3fn)}
+        hooks = {"plain": None, "qint8_axis0": B.quantize_on_save(torch.qint8, axis=0),
+                 "e4m3fn_axis0": B.quantize_on_save(torch.float8_e4m3fn, axis=0), "e4m3fn_cast": B.cast_on_save(torch.float8_e4m3fn)}
         for name, hook in hooks.items():  # warm-up: module loads, the arena, the pinned ring
             B.Snapshot.take(os.path.join(base, "warm"), app, _custom_tensor_prepare_func=hook)
             shutil.rmtree(os.path.join(base, "warm"))

@@ -379,7 +379,8 @@ def save_desc(
     cast; with ``wire_dtype`` torch.qint8/quint8 and ``qparams=(scale, zero_point)`` the pack kernel quantises and
     appends the 16-byte per-tensor trailer (T:serialization.py:278-310).  With ``axis`` instead of ``qparams`` the engine
     quantises per channel along ``axis`` (non-negative): ``wire_offset`` is then where the int body starts, behind the
-    8-byte axis header, and the channel parameters follow the body."""
+    8-byte axis header, and the channel parameters follow the body.  ``axis`` with a float8 ``wire_dtype`` is the
+    per-channel scaled float8 format, laid out the same way with one f32 scale per channel."""
     d = CopyDesc()
     sizes, strides = list(t.shape), list(t.stride())
     if len(sizes) > MAX_DIMS:
@@ -404,6 +405,8 @@ def save_desc(
             raise NativeError(-1, "quantising descriptors need qparams=(scale, zero_point) or an axis")
     else:
         d.dst_dtype = tsnap_dtype(wire_dtype or t.dtype)
+        if axis is not None:  # a float8 wire dtype: per-channel scaled float8
+            per_channel(d, list(t.shape), axis, wire_offset)
     d.src_space = _space_of(t)
     d.dst_space = SPACE_WIRE
     return d

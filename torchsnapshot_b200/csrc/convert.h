@@ -97,6 +97,22 @@ TSNAP_HD uint8_t fp8_from_f32(float f, uint32_t dt) { return dt == TSNAP_F8E4M3F
 
 TSNAP_HD float fp8_to_f32(uint8_t b, uint32_t dt) { return dt == TSNAP_F8E4M3FN ? fp8_e4m3fn_to_f32(b) : fp8_e5m2_to_f32(b); }
 
+// ---- per-channel scaled float8 ---------------------------------------------------------------------------------------
+// Largest finite value of each format.  An element x (as fp32) of a channel with scale s is stored as
+// float8(clamp(x / s, -FMAX, FMAX)) with an IEEE fp32 division, and restored as fp32(q) * s in fp32.
+TSNAP_HD float fp8_max(uint32_t dt) { return dt == TSNAP_F8E4M3FN ? 448.0f : 57344.0f; }
+TSNAP_HD uint8_t fp8_quantize(float x, float s, uint32_t dt) {
+    const float fmax = fp8_max(dt);
+#ifdef __CUDA_ARCH__
+    float y = __fdiv_rn(x, s);
+#else
+    float y = x / s;
+#endif
+    y = y < -fmax ? -fmax : (y > fmax ? fmax : y);
+    return fp8_from_f32(y, dt);
+}
+TSNAP_HD float fp8_dequantize(uint8_t q, uint32_t dt, float s) { return fp8_to_f32(q, dt) * s; }
+
 // ---- fp16 / bf16 <-> fp32 --------------------------------------------------------------------------------------------
 // Widening is exact (a signalling NaN keeps its bits); narrowing rounds to nearest even and keeps subnormals.
 TSNAP_HD float f16_to_f32(uint16_t h) {

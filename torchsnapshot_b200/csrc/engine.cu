@@ -631,13 +631,14 @@ static int plan_wave(tsnap_job* job, Wave& w) {
                 const uint64_t nt = tile_count(m);
                 if (nt == 0) continue;
                 const uint32_t mi = uint32_t(w.members.size());
-                if (m.mode == kModeQChannel) {
+                if (qchannel_mode(m.mode)) {
                     // a save runs statistics over the same tiles and finalises the parameters before the quantising pack
                     m.q_zero_point = int64_t(w.qch.size());
                     w.qch.push_back(nc.qc);
                     if (nc.qc.save) {
                         for (uint64_t t = 0; t < nt; ++t) w.tiles[kKernelQStats].push_back(Tile{mi, uint32_t(t)});
-                        for (uint64_t t = 0; t * kQChannelsPerTile < nc.qc.channels; ++t) w.tiles[kKernelQParams].push_back(Tile{mi, uint32_t(t)});
+                        const Kernel params = m.mode == kModeQChannelFp8 ? kKernelQParamsFp8 : kKernelQParams;
+                        for (uint64_t t = 0; t * kQChannelsPerTile < nc.qc.channels; ++t) w.tiles[params].push_back(Tile{mi, uint32_t(t)});
                         w.qkey_bytes += 16 * nc.qc.channels;
                     }
                 }
@@ -712,7 +713,7 @@ static int launch_wave(tsnap_job* job, Wave& w) {
     for (int k = 0; k < kKernelCount; ++k) {
         const Kernel kernel = Kernel(k);
         const Tile* d_tiles = reinterpret_cast<const Tile*>(d + seg[2 + k].off);
-        if (kernel == kKernelQStats || kernel == kKernelQParams || kernel == kKernelQChannel)
+        if (kernel >= kKernelQStats && kernel <= kKernelQChannelFp8)
             CUDA_TRY(launch_qchannel_kernel(kernel, d_members, d_qch, d_tiles, uint32_t(w.tiles[k].size()), d_qflag, eng->sm_count, eng->s_kernel));
         else
             CUDA_TRY(launch_kernel(kernel, d_members, d_tiles, d_maps, uint32_t(w.tiles[k].size()), eng->sm_count, eng->s_kernel));
@@ -1768,12 +1769,12 @@ static int add_member(tsnap_job* job, int32_t fi, const tsnap_copy_desc* d, bool
     uint64_t wire_lo = d->dst_addr, wire_end = 0;
     if (d->reserved == TSNAP_QSCHEME_PER_CHANNEL) {
         // the engine plans after this call returns: keep its own copy of the record
-        if (nc.qc.params + 16 * nc.qc.channels > f.nbytes) return set_err(TSNAP_EINVAL, "per-channel parameters exceed the file's wire image");
+        if (nc.qc.params + nc.qc.param_bytes * nc.qc.channels > f.nbytes) return set_err(TSNAP_EINVAL, "per-channel parameters exceed the file's wire image");
         job->qrecs.push_back(*reinterpret_cast<const tsnap_qchannel*>(uintptr_t(d->q_zero_point)));
         own.q_zero_point = int64_t(uintptr_t(&job->qrecs.back()));
         if (save) {
             wire_lo = nc.qc.body - 8;
-            wire_end = nc.qc.params + 16 * nc.qc.channels;
+            wire_end = nc.qc.params + nc.qc.param_bytes * nc.qc.channels;
         }
     } else if (save) {
         const bool quant = d->dst_dtype == TSNAP_QINT8 || d->dst_dtype == TSNAP_QUINT8;
@@ -2188,7 +2189,7 @@ int tsnap_consume(tsnap_engine* eng, const void* host_buf, uint64_t nbytes, cons
             NormalizedCopy nc;
             int rc = normalize_copy(members[i], uint64_t(uintptr_t(host_buf)), false, &nc, &err);
             if (rc == TSNAP_OK && members[i].reserved == TSNAP_QSCHEME_PER_CHANNEL &&
-                nc.qc.params - uint64_t(uintptr_t(host_buf)) + 16 * nc.qc.channels > nbytes)
+                nc.qc.params - uint64_t(uintptr_t(host_buf)) + nc.qc.param_bytes * nc.qc.channels > nbytes)
                 return set_err(TSNAP_EINVAL, "per-channel parameters exceed the buffer");
             if (rc == TSNAP_OK) rc = host_copy_all(nc, &err);
             if (rc != TSNAP_OK) return set_err(rc, err);
@@ -2321,7 +2322,7 @@ int tsnap_host_execute(const tsnap_copy_desc* members, int32_t n, void* wire_buf
         if (rc != TSNAP_OK) return set_err(rc, err);
         if (d.reserved == TSNAP_QSCHEME_PER_CHANNEL) {
             // three dependent passes over the whole member: one work item, run before the others
-            if (nc.qc.params - uint64_t(uintptr_t(wire_buf)) + 16 * nc.qc.channels > wire_nbytes)
+            if (nc.qc.params - uint64_t(uintptr_t(wire_buf)) + nc.qc.param_bytes * nc.qc.channels > wire_nbytes)
                 return set_err(TSNAP_EINVAL, "per-channel member exceeds the wire buffer");
             rc = host_copy_all(nc, &err);
             if (rc != TSNAP_OK) return set_err(rc, err);

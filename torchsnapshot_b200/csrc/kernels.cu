@@ -908,6 +908,19 @@ __device__ __forceinline__ void st_u64_any(char* p, uint64_t v) {
     }
     for (int i = 0; i < 8; ++i) p[i] = (char)(v >> (8 * i));
 }
+__device__ __forceinline__ uint32_t ld_u32_any(const char* p) {
+    if ((reinterpret_cast<uintptr_t>(p) & 3) == 0) return *reinterpret_cast<const uint32_t*>(p);
+    uint32_t v = 0;
+    for (int i = 3; i >= 0; --i) v = (v << 8) | (uint8_t)p[i];
+    return v;
+}
+__device__ __forceinline__ void st_u32_any(char* p, uint32_t v) {
+    if ((reinterpret_cast<uintptr_t>(p) & 3) == 0) {
+        *reinterpret_cast<uint32_t*>(p) = v;
+        return;
+    }
+    for (int i = 0; i < 4; ++i) p[i] = (char)(v >> (8 * i));
+}
 
 // The source elements of save chunk [e, e + n) as fp32 (the value the quantiser reads); 16 B loads when the chunk is
 // a full, 16 B-aligned piece of one dense run.
@@ -1067,7 +1080,9 @@ __global__ void __launch_bounds__(kLsuThreads) tsnap_qstats_kernel(const Member*
 }
 
 // finalises each channel's keys into (scale: f64, zero_point: i64) in place, copies them into the wire image and writes
-// the axis header; a NaN / Inf channel raises *nonfinite
+// the axis header; a NaN / Inf channel raises *nonfinite.  kFp8 (kModeQChannelFp8): the f32 scale of fp8_scale_of
+// instead, in the key slot and in the wire image.
+template <bool kFp8>
 __global__ void __launch_bounds__(kLsuThreads) tsnap_qparams_kernel(const Member* __restrict__ members, const QChannel* __restrict__ qch,
                                                                     const Tile* __restrict__ tiles, uint32_t ntiles, int* nonfinite) {
     for (uint32_t t = blockIdx.x; t < ntiles; t += gridDim.x) {
@@ -1078,7 +1093,18 @@ __global__ void __launch_bounds__(kLsuThreads) tsnap_qparams_kernel(const Member
         const uint64_t c0 = (uint64_t)tl.index * kQChannelsPerTile;
         const uint64_t c1 = c0 + kQChannelsPerTile < q.channels ? c0 + kQChannelsPerTile : q.channels;
         char* params = reinterpret_cast<char*>(q.params);
-        for (uint64_t c = c0 + threadIdx.x; c < c1; c += kLsuThreads) {
+        if constexpr (kFp8) {
+            for (uint64_t c = c0 + threadIdx.x; c < c1; c += kLsuThreads) {
+                int* k = reinterpret_cast<int*>(q.keys) + 2 * c;
+                float s;
+                if (!fp8_scale_of(k[0], k[1], m.dst_dtype, &s)) {
+                    *nonfinite = 1;
+                    s = __int_as_float(0x7fc00000);
+                }
+                k[0] = __float_as_int(s);  // the pack divides by it
+                st_u32_any(params + 4 * c, __float_as_uint(s));
+            }
+        } else for (uint64_t c = c0 + threadIdx.x; c < c1; c += kLsuThreads) {
             int* k = reinterpret_cast<int*>(q.keys) + 2 * c;
             double scale;
             int64_t zp;
@@ -1098,8 +1124,107 @@ __global__ void __launch_bounds__(kLsuThreads) tsnap_qparams_kernel(const Member
     }
 }
 
+// One kModeQChannelFp8 tile, [lo, hi) of the member's destination bytes; kDt is the float8 wire dtype.
+// Save: float8(clamp(x / s, -FMAX, FMAX)) with fp8_quantize's IEEE division, 16 elements and one 16 B store per thread
+// as in the int8 pack.  Restore: fp32(q) * s, converted once to the destination dtype.
+template <uint32_t kDt>
+__device__ __forceinline__ void qchannel_fp8_tile(const Member& m, const QChannel& q, uint64_t lo, uint64_t hi) {
+    if (q.save) {
+        const float* sk = reinterpret_cast<const float*>(q.keys);  // (s, unused) per channel, from tsnap_qparams_kernel<true>
+        char* db = reinterpret_cast<char*>(m.dst);
+        uint64_t ce;
+        uint32_t cn;
+        for (uint64_t k = threadIdx.x; qsave_chunk(m, lo, hi, k, &ce, &cn); k += kLsuThreads) {
+            float x[kQChunk];
+            qload_chunk(m, ce, cn, x);
+            uint64_t c, r;
+            qchan_at(q, m.dst + ce, &c, &r);
+            uint64_t loaded = ~uint64_t(0);
+            float s = 1.0f;
+            uint32_t o[4] = {0, 0, 0, 0};
+#pragma unroll
+            for (uint32_t i = 0; i < kQChunk; ++i) {
+                if (i < cn) {
+                    if (c != loaded) {
+                        s = sk[2 * c];
+                        loaded = c;
+                    }
+                    o[i >> 2] |= (uint32_t)fp8_quantize(x[i], s, kDt) << (8 * (i & 3));
+                    qchan_next(q, &c, &r);
+                }
+            }
+            if (cn == kQChunk) {
+                st_stream16(db + ce, make_uint4(o[0], o[1], o[2], o[3]));
+            } else {
+                for (uint32_t i = 0; i < cn; ++i) db[ce + i] = (char)(o[i >> 2] >> (8 * (i & 3)));
+            }
+        }
+        return;
+    }
+    const char* sb = reinterpret_cast<const char*>(m.src);
+    char* db = reinterpret_cast<char*>(m.dst);
+    const char* params = reinterpret_cast<const char*>(q.params);  // f32 scales at any alignment
+    bool aligned = (m.dst % m.dst_esz) == 0;
+    for (uint32_t i = 0; i < m.nouter; ++i) aligned = aligned && ((uint64_t)m.dstride[i] % m.dst_esz) == 0;
+    const uint64_t e0 = lo / m.dst_esz, e1 = hi / m.dst_esz;
+    if (m.nouter == 0 && m.dst_dtype != TSNAP_F64 && ((m.dst + e0 * m.dst_esz) & 15) == 0 && ((m.src + e0) & 3) == 0) {
+        // one dense run on both sides: 4 elements per thread and step, a 4-byte load and one 8 or 16-byte store
+        const uint64_t ngroups = (e1 - e0) / 4;
+        uint64_t loaded = ~uint64_t(0);
+        float s = 1.0f;
+        for (uint64_t g = threadIdx.x; g < ngroups; g += kLsuThreads) {
+            const uint64_t e = e0 + 4 * g;
+            const uint32_t w = *reinterpret_cast<const uint32_t*>(sb + e);
+            uint64_t c, r;
+            qchan_at(q, m.src + e, &c, &r);
+            float f[4];
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                if (c != loaded) {
+                    s = __uint_as_float(ld_u32_any(params + 4 * c));
+                    loaded = c;
+                }
+                f[i] = fp8_dequantize((uint8_t)(w >> (8 * i)), kDt, s);
+                qchan_next(q, &c, &r);
+            }
+            char* p = db + e * m.dst_esz;
+            if (m.dst_dtype == TSNAP_F32) {
+                *reinterpret_cast<float4*>(p) = make_float4(f[0], f[1], f[2], f[3]);
+            } else {
+                uint16_t h[4];
+#pragma unroll
+                for (int i = 0; i < 4; ++i) h[i] = f16_or_bf16_from_f32(f[i], m.dst_dtype);
+                *reinterpret_cast<uint2*>(p) = make_uint2(h[0] | ((uint32_t)h[1] << 16), h[2] | ((uint32_t)h[3] << 16));
+            }
+        }
+        if (threadIdx.x == 0) {  // the ragged tail (< 4 elements)
+            for (uint64_t e = e0 + 4 * ngroups; e < e1; ++e) {
+                uint64_t c, r;
+                qchan_at(q, m.src + e, &c, &r);
+                const float f = fp8_dequantize((uint8_t)sb[e], kDt, __uint_as_float(ld_u32_any(params + 4 * c)));
+                store_f32(db + e * m.dst_esz, m.dst_dtype, f, true);
+            }
+        }
+        return;
+    }
+    for (uint64_t e = e0 + (uint64_t)threadIdx.x * kQChunk; e < e1; e += (uint64_t)kLsuThreads * kQChunk) {
+        const uint32_t n = e1 - e < kQChunk ? (uint32_t)(e1 - e) : kQChunk;
+        QWalk w;
+        qwalk_at(m, e, w);
+        uint64_t c, r;
+        qchan_at(q, m.src + w.so + w.col, &c, &r);
+        for (uint32_t i = 0; i < n; ++i) {
+            const float s = __uint_as_float(ld_u32_any(params + 4 * c));
+            store_f32(db + w.dofs + w.col * m.dst_esz, m.dst_dtype, fp8_dequantize((uint8_t)sb[w.so + w.col], kDt, s), aligned);
+            if (qwalk_next(m, w)) qchan_at(q, m.src + w.so, &c, &r);
+            else qchan_next(q, &c, &r);
+        }
+    }
+}
+
 // torch's per-channel quantiser on the device (ATen/native/quantized/cuda/AffineQuantizer.cu): the same rounding as
-// quantize_elem, with the channel's parameters
+// quantize_elem, with the channel's parameters.  kFp8: the scaled float8 tiles of kModeQChannelFp8 instead.
+template <bool kFp8>
 __global__ void __launch_bounds__(kLsuThreads) tsnap_qchannel_kernel(const Member* __restrict__ members, const QChannel* __restrict__ qch,
                                                                      const Tile* __restrict__ tiles, uint32_t ntiles) {
     for (uint32_t t = blockIdx.x; t < ntiles; t += gridDim.x) {
@@ -1108,6 +1233,11 @@ __global__ void __launch_bounds__(kLsuThreads) tsnap_qchannel_kernel(const Membe
         const QChannel q = qch[m.q_zero_point];
         uint64_t lo, hi;
         tile_range_lsu(m, tl.index, &lo, &hi);
+        if constexpr (kFp8) {
+            if ((q.save ? m.dst_dtype : m.src_dtype) == TSNAP_F8E4M3FN) qchannel_fp8_tile<TSNAP_F8E4M3FN>(m, q, lo, hi);
+            else qchannel_fp8_tile<TSNAP_F8E5M2>(m, q, lo, hi);
+            continue;
+        }
         if (q.save) {
             const bool is_signed = m.dst_dtype == TSNAP_QINT8;
             const uint2* kp = reinterpret_cast<const uint2*>(q.keys);                       // (1 / scale: f32, zero_point: i32)
@@ -1237,7 +1367,8 @@ constexpr int kRowsSmem = kRingStages * kRingStageBytes + kRingStages * (int)siz
 // resident CTAs per SM of the three builds of the LSU kernel (kKernelLsu, kKernelLsuStrided, kKernelLsuTranspose), from
 // the occupancy calculator: each persistent grid is exactly one wave
 static int g_lsu_ctas_per_sm[3] = {3, 2, 6};
-static int g_qchannel_ctas_per_sm[3] = {2, 2, 2};  // kKernelQStats, kKernelQParams, kKernelQChannel (from the occupancy calculator)
+// kKernelQStats .. kKernelQChannelFp8 (from the occupancy calculator)
+static int g_qchannel_ctas_per_sm[5] = {2, 2, 2, 2, 2};
 
 cudaError_t init_kernels() {
     cudaError_t e = cudaFuncSetAttribute(tsnap_bulk_copy_kernel<kRingStages, kRingStageBytes>, cudaFuncAttributeMaxDynamicSharedMemorySize, kBulkSmem);
@@ -1249,8 +1380,10 @@ cudaError_t init_kernels() {
         if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, tsnap_lsu_copy_kernel<2>, kLsuThreads, 0) == cudaSuccess && n > 0) g_lsu_ctas_per_sm[1] = n;
         if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, tsnap_lsu_copy_kernel<6>, kLsuThreads, 0) == cudaSuccess && n > 0) g_lsu_ctas_per_sm[2] = n;
         if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, tsnap_qstats_kernel, kLsuThreads, 0) == cudaSuccess && n > 0) g_qchannel_ctas_per_sm[0] = n;
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, tsnap_qparams_kernel, kLsuThreads, 0) == cudaSuccess && n > 0) g_qchannel_ctas_per_sm[1] = n;
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, tsnap_qchannel_kernel, kLsuThreads, 0) == cudaSuccess && n > 0) g_qchannel_ctas_per_sm[2] = n;
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, tsnap_qparams_kernel<false>, kLsuThreads, 0) == cudaSuccess && n > 0) g_qchannel_ctas_per_sm[1] = n;
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, tsnap_qparams_kernel<true>, kLsuThreads, 0) == cudaSuccess && n > 0) g_qchannel_ctas_per_sm[2] = n;
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, tsnap_qchannel_kernel<false>, kLsuThreads, 0) == cudaSuccess && n > 0) g_qchannel_ctas_per_sm[3] = n;
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, tsnap_qchannel_kernel<true>, kLsuThreads, 0) == cudaSuccess && n > 0) g_qchannel_ctas_per_sm[4] = n;
     }
     return e;
 }
@@ -1279,8 +1412,10 @@ cudaError_t launch_qchannel_kernel(Kernel k, const Member* d_members, const QCha
     if (grid > ntiles) grid = ntiles;
     switch (k) {
         case kKernelQStats: tsnap_qstats_kernel<<<grid, kLsuThreads, 0, stream>>>(d_members, d_qch, d_tiles, ntiles); break;
-        case kKernelQParams: tsnap_qparams_kernel<<<grid, kLsuThreads, 0, stream>>>(d_members, d_qch, d_tiles, ntiles, nonfinite); break;
-        default: tsnap_qchannel_kernel<<<grid, kLsuThreads, 0, stream>>>(d_members, d_qch, d_tiles, ntiles); break;
+        case kKernelQParams: tsnap_qparams_kernel<false><<<grid, kLsuThreads, 0, stream>>>(d_members, d_qch, d_tiles, ntiles, nonfinite); break;
+        case kKernelQParamsFp8: tsnap_qparams_kernel<true><<<grid, kLsuThreads, 0, stream>>>(d_members, d_qch, d_tiles, ntiles, nonfinite); break;
+        case kKernelQChannelFp8: tsnap_qchannel_kernel<true><<<grid, kLsuThreads, 0, stream>>>(d_members, d_qch, d_tiles, ntiles); break;
+        default: tsnap_qchannel_kernel<false><<<grid, kLsuThreads, 0, stream>>>(d_members, d_qch, d_tiles, ntiles); break;
     }
     return cudaGetLastError();
 }

@@ -13,7 +13,9 @@ enum Kernel {
     kKernelRowsTma,       // kModeRowsTma: tensor-map boxes of many short runs (transpose_tma.cu)
     kKernelQStats,        // kModeQChannel saves: per-channel min / max of the source into the wave's key slots
     kKernelQParams,       // kModeQChannel saves: keys -> (scale, zero_point), the wire image's parameters and axis header
+    kKernelQParamsFp8,    // kModeQChannelFp8 saves: keys -> f32 scale, the wire image's scales and axis header
     kKernelQChannel,      // kModeQChannel: quantising pack (16 B of int8 per thread) / dequantising scatter
+    kKernelQChannelFp8,   // kModeQChannelFp8: scaled float8 pack (16 B of float8 per thread) / dequantising scatter
     kKernelLsu,           // kModeContig, kModeCast: 3 CTAs/SM, 80 registers: unaligned dense runs 0.76, fp32 -> bf16 casts 0.87
     kKernelLsuStrided,    // kModeStrided: 2 CTAs/SM, 128 registers: the strided gather keeps 8 independent 16 B loads per
                           // thread in flight without spilling (0.68 on 128 B runs)
@@ -36,6 +38,7 @@ inline Kernel kernel_of(uint32_t mode) {
         case kModeTranspose: return kKernelLsuTranspose;
         case kModeTransposeTma: return kKernelTransposeTma;
         case kModeQChannel: return kKernelQChannel;
+        case kModeQChannelFp8: return kKernelQChannelFp8;
         default: return kKernelLsu;  // kModeContig, kModeCast
     }
 }
@@ -48,7 +51,7 @@ cudaError_t init_kernels();
 cudaError_t launch_kernel(Kernel k, const Member* d_members, const Tile* d_tiles, const TmaPair* d_maps, uint32_t ntiles,
                           int sm_count, cudaStream_t stream);
 
-// launch_kernel for the three kModeQChannel kernels: `d_qch` is the wave's QChannel table, `nonfinite` a word the
+// launch_kernel for the kModeQChannel / kModeQChannelFp8 kernels (kKernelQStats .. kKernelQChannelFp8): `d_qch` is the wave's QChannel table, `nonfinite` a word the
 // parameter kernel sets when a channel holds a NaN or Inf
 cudaError_t launch_qchannel_kernel(Kernel k, const Member* d_members, const QChannel* d_qch, const Tile* d_tiles, uint32_t ntiles,
                                    int* nonfinite, int sm_count, cudaStream_t stream);

@@ -23,8 +23,9 @@ bool cast_supported(int s, int d) {
     return (is_float(s) || is_fp8_dtype(s)) && (is_float(d) || is_fp8_dtype(d));
 }
 
-// TSNAP_QSCHEME_PER_CHANNEL: float -> quantised on save, and back on restore
-static bool per_channel_supported(int s, int d) { return (is_float(s) && is_quant(d)) || (is_quant(s) && is_float(d)); }
+// TSNAP_QSCHEME_PER_CHANNEL: float -> int8 or scaled float8 on save, and back on restore
+static bool per_channel_narrow(int dt) { return is_quant(dt) || is_fp8_dtype(uint32_t(dt)); }
+static bool per_channel_supported(int s, int d) { return (is_float(s) && per_channel_narrow(d)) || (per_channel_narrow(s) && is_float(d)); }
 
 static inline uint64_t lowbit(uint64_t x) { return x & (~x + 1); }
 
@@ -65,7 +66,8 @@ int normalize_copy(const tsnap_copy_desc& d, uint64_t wire_base, bool allow_bulk
     const bool quant = is_quant(d.dst_dtype);
     if (!per_channel && quant && (d.dst_space != TSNAP_SPACE_WIRE || !(d.q_scale > 0)))
         return fail(TSNAP_EINVAL, "quantising copies need a WIRE destination and q_scale > 0");
-    if (per_channel && (quant ? d.dst_space : d.src_space) != TSNAP_SPACE_WIRE)
+    const bool pc_save = per_channel && per_channel_narrow(d.dst_dtype);  // a per-channel save (else a restore)
+    if (per_channel && (pc_save ? d.dst_space : d.src_space) != TSNAP_SPACE_WIRE)
         return fail(TSNAP_EINVAL, "per-channel copies keep the quantised side in WIRE space");
 
     // logical shape; C-contiguous element strides for a WIRE destination
@@ -90,7 +92,7 @@ int normalize_copy(const tsnap_copy_desc& d, uint64_t wire_base, bool allow_bulk
         const uint64_t period = uint64_t(r.channels) * uint64_t(r.inner);
         if (r.params_addr < r.body_addr || (r.params_addr - r.body_addr) % period != 0)
             return fail(TSNAP_EINVAL, "tsnap_qchannel: the body is not a whole number of channels x inner elements");
-        if (quant) {
+        if (pc_save) {
             if (r.body_addr < 8 || d.dst_addr != r.body_addr || r.params_addr != r.body_addr + numel)
                 return fail(TSNAP_EINVAL, "tsnap_qchannel: a per-channel save writes the whole piece: header at body - 8, "
                                           "body at dst_addr, parameters right behind it");
@@ -99,14 +101,15 @@ int normalize_copy(const tsnap_copy_desc& d, uint64_t wire_base, bool allow_bulk
             uint64_t last = d.src_addr;
             for (int i = 0; i < d.ndim; ++i) last += uint64_t(d.sizes[i] - 1) * uint64_t(d.src_strides[i]);
             if (d.src_addr < r.body_addr || last >= r.params_addr)
-                return fail(TSNAP_EINVAL, "tsnap_qchannel: the member reads outside the piece's int body");
+                return fail(TSNAP_EINVAL, "tsnap_qchannel: the member reads outside the piece's body");
         }
         out->qc.body = r.body_addr + wire_base;
         out->qc.params = r.params_addr + wire_base;
         out->qc.channels = uint64_t(r.channels);
         out->qc.inner = uint64_t(r.inner);
         out->qc.axis = r.axis;
-        out->qc.save = quant ? 1 : 0;
+        out->qc.save = pc_save ? 1 : 0;
+        out->qc.param_bytes = is_fp8_dtype(uint32_t(pc_save ? d.dst_dtype : d.src_dtype)) ? 4 : 16;
     }
     if (numel == 0) return TSNAP_OK;
 
@@ -174,7 +177,7 @@ int normalize_copy(const tsnap_copy_desc& d, uint64_t wire_base, bool allow_bulk
 
     if (cast) {
         if (per_channel) {
-            m.mode = kModeQChannel;
+            m.mode = out->qc.param_bytes == 4 ? kModeQChannelFp8 : kModeQChannel;
             m.shift = 0;
         }
         out->m[0] = m;
@@ -306,14 +309,17 @@ void host_copy_range(const Member& m, uint64_t lo, uint64_t hi) {
 
 // ---- per-channel quantisation on the host ------------------------------------------------------------------
 // The three passes of the device (statistics, parameters, quantising pack) in one sequential sweep each, with the same
-// rules: the element as fp32, channel keys that start at 0, the parameters of qparams_of, torch's CPU quantiser.
+// rules: the element as fp32, channel keys that start at 0, the parameters of qparams_of, torch's CPU quantiser.  A
+// float8 wire (kModeQChannelFp8) takes fp8_scale_of, fp8_quantize and fp8_dequantize instead, with f32 scales.
 int host_qchannel(const Member& m, const QChannel& q, std::string* err) {
     const char* src = reinterpret_cast<const char*>(uintptr_t(m.src));
     char* dst = reinterpret_cast<char*>(uintptr_t(m.dst));
     const uint64_t n = m.bytes / m.dst_esz;
     char* params = reinterpret_cast<char*>(uintptr_t(q.params));
     auto channel = [&](uint64_t wire_addr) { return ((wire_addr - q.body) / q.inner) % q.channels; };
-    const bool is_signed = (q.save ? m.dst_dtype : m.src_dtype) == TSNAP_QINT8;
+    const bool fp8 = m.mode == kModeQChannelFp8;
+    const uint32_t wire_dt = q.save ? m.dst_dtype : m.src_dtype;
+    const bool is_signed = wire_dt == TSNAP_QINT8;
     if (!q.save) {
         for (uint64_t e = 0; e < n; ++e) {
             const uint64_t row = e / m.inner, col = e % m.inner;
@@ -321,12 +327,20 @@ int host_qchannel(const Member& m, const QChannel& q, std::string* err) {
             outer_offsets(m, row, &so, &dofs);
             const uint64_t a = m.src + uint64_t(so) + col;
             const uint64_t c = channel(a);
-            double scale;
-            int64_t zp;
-            std::memcpy(&scale, params + 8 * c, 8);
-            std::memcpy(&zp, params + 8 * (q.channels + c), 8);
             const uint8_t raw = *reinterpret_cast<const uint8_t*>(uintptr_t(a));
-            store_f32(dst + dofs + col * m.dst_esz, m.dst_dtype, dequantize(raw, is_signed, zp, scale), false);
+            float f;
+            if (fp8) {
+                float s;
+                std::memcpy(&s, params + 4 * c, 4);
+                f = fp8_dequantize(raw, wire_dt, s);
+            } else {
+                double scale;
+                int64_t zp;
+                std::memcpy(&scale, params + 8 * c, 8);
+                std::memcpy(&zp, params + 8 * (q.channels + c), 8);
+                f = dequantize(raw, is_signed, zp, scale);
+            }
+            store_f32(dst + dofs + col * m.dst_esz, m.dst_dtype, f, false);
         }
         return TSNAP_OK;
     }
@@ -340,30 +354,35 @@ int host_qchannel(const Member& m, const QChannel& q, std::string* err) {
         kmin[c] = std::min(kmin[c], k);
         kmax[c] = std::max(kmax[c], k);
     }
-    std::vector<double> scale(q.channels);
-    std::vector<int64_t> zp(q.channels);
+    std::vector<double> scale(fp8 ? 0 : q.channels);
+    std::vector<int64_t> zp(fp8 ? 0 : q.channels);
+    std::vector<float> fp8_scale(fp8 ? q.channels : 0);
     for (uint64_t c = 0; c < q.channels; ++c) {
-        if (!qparams_of(kmin[c], kmax[c], is_signed, &scale[c], &zp[c])) {
+        if (fp8 ? !fp8_scale_of(kmin[c], kmax[c], wire_dt, &fp8_scale[c]) : !qparams_of(kmin[c], kmax[c], is_signed, &scale[c], &zp[c])) {
             if (err) *err = "per-channel quantisation: channel " + std::to_string(c) + " holds a NaN or Inf";
             return TSNAP_EINVAL;
         }
     }
     std::memcpy(reinterpret_cast<char*>(uintptr_t(q.body)) - 8, &q.axis, 8);
-    std::memcpy(params, scale.data(), 8 * q.channels);
-    std::memcpy(params + 8 * q.channels, zp.data(), 8 * q.channels);
+    if (fp8) {
+        std::memcpy(params, fp8_scale.data(), 4 * q.channels);
+    } else {
+        std::memcpy(params, scale.data(), 8 * q.channels);
+        std::memcpy(params + 8 * q.channels, zp.data(), 8 * q.channels);
+    }
     for (uint64_t e = 0; e < n; ++e) {
         const uint64_t row = e / m.inner, col = e % m.inner;
         int64_t so, dofs;
         outer_offsets(m, row, &so, &dofs);
         const float x = load_f32(src + so + col * m.src_esz, m.src_dtype, false);
         const uint64_t c = channel(m.dst + uint64_t(dofs) + col);
-        reinterpret_cast<uint8_t*>(dst + dofs)[col] = quantize_elem(x, scale[c], zp[c], is_signed);
+        reinterpret_cast<uint8_t*>(dst + dofs)[col] = fp8 ? fp8_quantize(x, fp8_scale[c], wire_dt) : quantize_elem(x, scale[c], zp[c], is_signed);
     }
     return TSNAP_OK;
 }
 
 int host_copy_all(const NormalizedCopy& nc, std::string* err) {
-    if (nc.n == 1 && nc.m[0].mode == kModeQChannel) return host_qchannel(nc.m[0], nc.qc, err);
+    if (nc.n == 1 && qchannel_mode(nc.m[0].mode)) return host_qchannel(nc.m[0], nc.qc, err);
     for (int k = 0; k < nc.n; ++k) host_copy_range(nc.m[k], 0, nc.m[k].bytes);
     return TSNAP_OK;
 }

@@ -38,7 +38,9 @@ enum Mode : uint32_t {
                        // enough for the copy engine: one cp.async.bulk per run (or one per stage on a dense side)
     kModeQChannel = 8,  // kModeCast of a TSNAP_QSCHEME_PER_CHANNEL descriptor: float -> QINT8/QUINT8 (save) or back
                         // (restore) with per-channel parameters; q_zero_point indexes the wave's QChannel table
+    kModeQChannelFp8 = 9,  // kModeQChannel with a float8 wire dtype: per-channel scaled float8 (one f32 scale per channel)
 };
+TSNAP_HD bool qchannel_mode(uint32_t mode) { return mode == kModeQChannel || mode == kModeQChannelFp8; }
 constexpr uint32_t kRowsSrcDense = 1;  // Member.shift bits in kModeRows: consecutive runs are adjacent on that side
 constexpr uint32_t kRowsDstDense = 2;
 constexpr uint64_t kRowsMinRun = 256;  // shorter runs stay on the LSU path (one copy-engine request per run does not pay)
@@ -47,17 +49,17 @@ constexpr uint64_t kRowsMinRun = 256;  // shorter runs stay on the LSU path (one
 // The channel of the wire element at address a is ((a - body) / inner) % channels.
 struct alignas(16) QChannel {
     uint64_t body;      // first int element of the piece
-    uint64_t params;    // scales[channels] (f64), then zero_points[channels] (i64)
+    uint64_t params;    // scales[channels] (f64), then zero_points[channels] (i64); float8: scales[channels] (f32)
     uint64_t channels;
     uint64_t inner;
     int64_t axis;
     uint64_t keys;      // save: 16 B per channel in the launch table, zeroed in stream order before the wave: 8 B per
                         // channel of running (min, max) keys of the statistics pass, which the parameter pass replaces by
-                        // (1 / scale: f32, zero_point: i32) for the quantising pack, then the scales (f64).  (The wire
-                        // image's parameter area cannot hold them: it follows a body of any length, so it is not even
-                        // 4 B aligned in general.)
-    uint32_t save;      // 1: float -> int (statistics, parameters, header), 0: int -> float
-    uint32_t pad;
+                        // (1 / scale: f32, zero_point: i32) for the quantising pack, then the scales (f64); float8
+                        // replaces the keys by (scale: f32, unused).  (The wire image's parameter area cannot hold them:
+                        // it follows a body of any length, so it is not even 4 B aligned in general.)
+    uint32_t save;      // 1: float -> int / float8 (statistics, parameters, header), 0: back to float
+    uint32_t param_bytes;  // parameter bytes per channel in the wire image: 16 (int8), 4 (float8)
 };
 constexpr uint32_t kQChannelsPerTile = 8192;  // channels per tile of the header/parameter kernels
 
@@ -260,6 +262,20 @@ TSNAP_HD bool qparams_of(int32_t kmin, int32_t kmax, bool is_signed, double* sca
         if (*scale == 0.0) *scale = 1.0;
         *zp = (int64_t)rint(-lo / *scale);  // round half to even (default rounding mode)
     }
+    return true;
+}
+// Scale of one per-channel scaled float8 channel from its (min, max) keys: s = amax / FMAX as an IEEE fp32 division,
+// 1 when that is 0 (an all-zero channel, or an amax so small that s underflows); false on NaN / Inf
+TSNAP_HD bool fp8_scale_of(int32_t kmin, int32_t kmax, uint32_t dt, float* s) {
+    if (kmax > kQKeyMax || kmin < kQKeyMin) return false;
+    const float lo = qkey_value(kmin), hi = qkey_value(kmax);
+    const float amax = hi > -lo ? hi : -lo;
+#ifdef __CUDA_ARCH__
+    *s = __fdiv_rn(amax, fp8_max(dt));
+#else
+    *s = amax / fp8_max(dt);
+#endif
+    if (*s == 0.0f) *s = 1.0f;
     return true;
 }
 

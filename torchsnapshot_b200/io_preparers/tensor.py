@@ -20,14 +20,15 @@ import torch
 from .. import _native
 from ..io_types import BufferConsumer, BufferStager, BufferType, Future, ReadReq, WriteReq
 from ..manifest import ChunkedTensorEntry, TensorEntry
-from ..native_plan import RAW, describe_consumer, describe_stager, entry_nbytes, raw_castable
-from ..prepare import _FLOATS, PER_CHANNEL_QTENSOR, PER_TENSOR_QTENSOR, PerChannel, fused_quant_of
+from ..native_plan import PER_CHANNEL, RAW, describe_consumer, describe_stager, entry_nbytes, raw_castable
+from ..prepare import _FLOATS, FP8_MAX, PER_CHANNEL_FP8, PER_CHANNEL_QTENSOR, PER_TENSOR_QTENSOR, PerChannel, fused_quant_of
 from ..serialization import (
     RAW_DTYPES,
     SUPPORTED_QUANTIZED_DTYPES,
     Serializer,
     dtype_to_element_size,
     dtype_to_string,
+    per_channel_fp8_from_bytes,
     per_channel_qtensor_from_bytes,
     per_tensor_qtensor_from_bytes,
     string_to_dtype,
@@ -64,7 +65,7 @@ class TensorBufferStager(BufferStager):
         self._tensor_prepare_func = _tensor_prepare_func
         # (qdtype, scale, zero_point) when the entry is a quantise-on-save one, a PerChannel for a per-channel one: the
         # pack kernel quantises
-        quantised = entry.serializer in (PER_TENSOR_QTENSOR, PER_CHANNEL_QTENSOR)
+        quantised = entry.serializer in (PER_TENSOR_QTENSOR,) + PER_CHANNEL
         self.qparams = fused_quant_of(_tensor_prepare_func, tensor) if quantised else None
 
     # ---- engine-facing description ------------------------------------------------------------
@@ -127,6 +128,8 @@ class TensorBufferConsumer(BufferConsumer):
             return per_tensor_qtensor_from_bytes(bytes(buf), string_to_dtype(entry.dtype), list(entry.shape))
         if entry.serializer == PER_CHANNEL_QTENSOR:
             return per_channel_qtensor_from_bytes(bytes(buf), string_to_dtype(entry.dtype), list(entry.shape))
+        if entry.serializer == PER_CHANNEL_FP8:  # the dequantised fp32 tensor
+            return per_channel_fp8_from_bytes(bytes(buf), string_to_dtype(entry.dtype), list(entry.shape))
         raise ValueError(f"Unrecognized serializer: {entry.serializer}.")
 
     async def consume_buffer(self, buf: bytes, executor: Optional[Executor] = None) -> None:
@@ -148,7 +151,8 @@ class TensorBufferConsumer(BufferConsumer):
 
 
 class _DecodingConsumer(BufferConsumer):
-    """Decodes a quantised entry into a new quantised tensor (read without an in-place target)."""
+    """Decodes a quantised entry into a new tensor (read without an in-place target): a quantised tensor for int8, the
+    dequantised fp32 tensor for scaled float8."""
 
     def __init__(self, entry: TensorEntry, fut: Future) -> None:
         self.entry = entry
@@ -187,7 +191,8 @@ class TensorIOPreparer:
         serializer = RAW if traced.dtype in RAW_DTYPES else PICKLED
         quant = fused_quant_of(_tensor_prepare_func, tensor) if _tensor_prepare_func is not None else None
         if isinstance(quant, PerChannel):
-            serializer = PER_CHANNEL_QTENSOR  # axis header + int_repr + per-channel parameters, produced by the engine
+            # axis header + int_repr or float8 bytes + per-channel parameters, produced by the engine
+            serializer = PER_CHANNEL_FP8 if quant.dtype in FP8_MAX else PER_CHANNEL_QTENSOR
         elif quant is not None:
             serializer = PER_TENSOR_QTENSOR  # int_repr + 16-byte trailer, produced by the pack kernel
         entry = TensorEntry(
@@ -208,7 +213,7 @@ class TensorIOPreparer:
     def can_load_inplace(entry: Union[TensorEntry, ChunkedTensorEntry], obj: Any) -> bool:
         if not isinstance(obj, torch.Tensor) or list(entry.shape) != list(obj.shape):
             return False
-        if getattr(entry, "serializer", None) in (PER_TENSOR_QTENSOR, PER_CHANNEL_QTENSOR) and obj.dtype in _FLOATS:
+        if getattr(entry, "serializer", None) in (PER_TENSOR_QTENSOR,) + PER_CHANNEL and obj.dtype in _FLOATS:
             return True  # dequantised into the float tensor it was quantised from (tensor_copy)
         return string_to_dtype(entry.dtype) == obj.dtype
 
@@ -226,8 +231,8 @@ class TensorIOPreparer:
         tensor_out: Optional[torch.Tensor] = None,
         buffer_size_limit_bytes: Optional[int] = None,
     ) -> Tuple[List[ReadReq], Future[torch.Tensor]]:
-        if entry.serializer == PER_CHANNEL_QTENSOR and (tensor_out is None or not cls.can_load_inplace(entry, tensor_out)):
-            # no float target: the result is the decoded quantised tensor
+        if entry.serializer in PER_CHANNEL and (tensor_out is None or not cls.can_load_inplace(entry, tensor_out)):
+            # no float target: the result is the decoded tensor (quantised for int8, dequantised fp32 for float8)
             fut: Future[torch.Tensor] = Future()
             return [ReadReq(path=entry.location, byte_range=entry.byte_range_tuple, buffer_consumer=_DecodingConsumer(entry, fut))], fut
         if tensor_out is None or not cls.can_load_inplace(entry, tensor_out):

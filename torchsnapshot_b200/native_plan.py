@@ -15,7 +15,7 @@ from typing import Any, List, Optional, Tuple
 import torch
 
 from . import _native
-from .prepare import _CASTABLE, _FLOATS, PER_CHANNEL_QTENSOR, PER_TENSOR_QTENSOR, PerChannel, fused_cast_of
+from .prepare import _CASTABLE, _FLOATS, PER_CHANNEL_FP8, PER_CHANNEL_QTENSOR, PER_TENSOR_QTENSOR, PerChannel, fused_cast_of
 from .serialization import RAW_DTYPES, Serializer, dtype_to_element_size, string_to_dtype
 
 RAW = Serializer.BUFFER_PROTOCOL.value
@@ -24,17 +24,22 @@ _DTYPES = {str(dt): dt for dt in RAW_DTYPES}
 Described = Tuple[List["_native.CopyDesc"], List[torch.Tensor], int]  # descriptors, keep-alive, wire bytes
 
 
+PER_CHANNEL = (PER_CHANNEL_QTENSOR, PER_CHANNEL_FP8)  # serializers of the per-channel formats
+_PARAM_BYTES = {PER_CHANNEL_QTENSOR: 16, PER_CHANNEL_FP8: 4}  # bytes of parameters per channel
+
+
 def entry_nbytes(entry: Any, axis: Optional[int] = None) -> int:
     """Payload size of a tensor entry.  A per-tensor quantised one carries ``[q_scale: double][q_zero_point: int64]``
     behind the int_repr bytes (T:serialization.py:278-310); a per-channel one ``[axis: int64]`` before them and, given
-    the axis (only the file records it), ``[scales: f64 x C][zero_points: i64 x C]`` behind them."""
+    the axis (only the file records it), its parameters behind them: ``[scales: f64 x C][zero_points: i64 x C]`` for
+    int8, ``[scales: f32 x C]`` for float8."""
     n = dtype_to_element_size(string_to_dtype(entry.dtype))
     for s in entry.shape:
         n *= s
     if entry.serializer == PER_TENSOR_QTENSOR:
         n += 16
-    elif entry.serializer == PER_CHANNEL_QTENSOR:
-        n += 8 + (16 * entry.shape[axis] if axis is not None else 0)
+    elif entry.serializer in PER_CHANNEL:
+        n += 8 + (_PARAM_BYTES[entry.serializer] * entry.shape[axis] if axis is not None else 0)
     return n
 
 
@@ -82,10 +87,10 @@ def _describe_tensor_stager(st: Any, offset: int, clones: Optional[HostCloneBudg
         return None
     t = tensor.detach()
     # quantise-on-save (prepare.quantize_on_save): the stager computed the parameters once, when it was created
-    q = getattr(st, "qparams", None) if serializer in (PER_TENSOR_QTENSOR, PER_CHANNEL_QTENSOR) else None
+    q = getattr(st, "qparams", None) if serializer in (PER_TENSOR_QTENSOR,) + PER_CHANNEL else None
     wire_dtype = qparams = axis = None
     if isinstance(q, PerChannel):
-        # the engine writes the axis header, the int body behind it and the channel parameters behind the body
+        # the engine writes the axis header, the int or float8 body behind it and the channel parameters behind the body
         wire_dtype, axis, nbytes, offset = q.dtype, q.axis, entry_nbytes(entry, q.axis), offset + 8
     elif q is not None:
         # the pack kernel writes int_repr + the 16-byte trailer
@@ -151,7 +156,7 @@ def _describe_tensor_consumer(c: Any, offset: int, root: Optional[str] = None, b
     entry = getattr(c, "entry", None)
     serializer = getattr(entry, "serializer", None)
     raw = serializer == RAW and entry.dtype in _DTYPES
-    if not raw and serializer != PER_CHANNEL_QTENSOR:
+    if not raw and serializer not in PER_CHANNEL:
         return None
     shape = list(entry.shape)
     regions = getattr(c, "overlapping_regions", None)

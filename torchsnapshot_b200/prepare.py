@@ -75,10 +75,14 @@ def fused_cast_of(func, tensor: torch.Tensor) -> Optional[torch.dtype]:
 
 PER_TENSOR_QTENSOR = "per_tensor_qtensor"  # TensorEntry.serializer of the reference's per-tensor format (T:serialization.py:278-310)
 PER_CHANNEL_QTENSOR = "per_channel_qtensor"  # ... and of its per-channel format (T:serialization.py:366-477)
+# this package's per-channel scaled float8 format: [axis: int64][fp8 body, C order][scales: float32 x C]
+PER_CHANNEL_FP8 = "per_channel_fp8"
+FP8_MAX = {torch.float8_e4m3fn: 448.0, torch.float8_e5m2: 57344.0}  # largest finite value of each format
 
 
 class PerChannel:
-    """What a per-channel quantise-on-save hook reports for a tensor: wire dtype and the (non-negative) axis."""
+    """What a per-channel quantise-on-save hook reports for a tensor: wire dtype (qint8, quint8 or a float8 format)
+    and the (non-negative) axis."""
 
     def __init__(self, dtype: torch.dtype, axis: int) -> None:
         self.dtype, self.axis = dtype, axis
@@ -106,6 +110,34 @@ def per_channel_qparams(t: torch.Tensor, dtype: torch.dtype, axis: int) -> "tupl
     return scale, zp
 
 
+def _channel_view(s: torch.Tensor, ndim: int, axis: int) -> torch.Tensor:
+    shape = [1] * ndim
+    shape[axis] = -1
+    return s.view(shape)
+
+
+def per_channel_fp8(t: torch.Tensor, dtype: torch.dtype, axis: int) -> "tuple[torch.Tensor, torch.Tensor]":
+    """The scaled float8 rule of ``quantize_on_save(float8 dtype, axis=k)``, computed by torch: (q: ``dtype`` tensor of
+    ``t``'s shape, scales: float32 of ``shape[axis]``).  The engine computes the same bytes on the device or host while
+    it packs.  Divisions are tensor / tensor, IEEE on the CPU and on CUDA (a Python-scalar divisor would become a
+    reciprocal multiplication on CUDA)."""
+    fmax = FP8_MAX[dtype]
+    x = t.detach().float()  # fp64 rounds to fp32 first
+    flat = x.movedim(axis, 0).reshape(x.shape[axis], -1)
+    if not bool(torch.isfinite(flat).all()):
+        raise ValueError("per-channel quantisation: a channel holds a NaN or Inf")
+    amax = flat.abs().amax(1)
+    s = amax / torch.full_like(amax, fmax)
+    s = torch.where(s == 0, torch.ones_like(s), s)  # all-zero channels, and amax so small that s underflows
+    q = (x / _channel_view(s, x.dim(), axis)).clamp(-fmax, fmax).to(dtype)
+    return q, s
+
+
+def dequantize_fp8(q: torch.Tensor, scales: torch.Tensor, axis: int) -> torch.Tensor:
+    """The restore half of the rule: ``q.float() * s`` in fp32; a restore converts this once to the target dtype."""
+    return q.float() * _channel_view(scales.float().to(q.device), q.dim(), axis)
+
+
 def quantize_on_save(dtype: torch.dtype = torch.qint8, qparams: Optional[Callable[[str, torch.Tensor], "tuple[float, int]"]] = None,
                      only: Optional[str] = None, axis: Optional[int] = None) -> Callable[[str, torch.Tensor, bool], torch.Tensor]:
     """A ``_custom_tensor_prepare_func`` that stores floating-point tensors per-tensor affine quantised
@@ -123,9 +155,22 @@ def quantize_on_save(dtype: torch.dtype = torch.qint8, qparams: Optional[Callabl
     with the default rule applied to each channel.  It applies to floating-point tensors with ``ndim >= 2`` and
     ``ndim > k`` and at least one element; 1-d tensors (biases, norms) are stored unchanged, since 16 bytes of
     parameters per channel would outweigh them.  The engine computes the parameters while it packs; a channel
-    holding a NaN or Inf fails the take."""
+    holding a NaN or Inf fails the take.
+
+    ``dtype`` ``torch.float8_e4m3fn`` or ``torch.float8_e5m2`` (``axis`` required) stores the same tensors as float8
+    with one fp32 scale per channel (``per_channel_fp8`` states the rule), in this package's format
+    ``[axis: int64][fp8 bytes][scales: float32 x C]``: a state such as Adam's ``exp_avg_sq``, whose magnitudes span
+    many orders, keeps every channel in float8's range.  Float8 sources are stored unchanged, and restoring into a
+    floating-point tensor dequantises on the engine; ``read_object`` gives the dequantised fp32 tensor."""
+    if dtype in FP8_MAX:
+        if axis is None:
+            raise ValueError("quantize_on_save: float8 needs axis=k (per-channel scales); cast_on_save(dtype) stores an "
+                             "unscaled float8 cast")
+        if qparams is not None:
+            raise ValueError("quantize_on_save: float8 per-channel scales are computed by the engine, not by qparams")
+        return _quantize_per_channel_on_save(dtype, int(axis), only)
     if dtype not in (torch.qint8, torch.quint8):
-        raise ValueError("quantize_on_save supports torch.qint8 and torch.quint8")
+        raise ValueError("quantize_on_save supports torch.qint8, torch.quint8, torch.float8_e4m3fn and torch.float8_e5m2")
     if axis is not None:
         if qparams is not None:
             raise ValueError("quantize_on_save: axis (per-channel) does not take caller-supplied qparams")
@@ -183,6 +228,8 @@ def _quantize_per_channel_on_save(dtype: torch.dtype, axis: int, only: Optional[
             return tensor
         if tracing:
             return _Traced(tensor.shape, dtype)
+        if dtype in FP8_MAX:  # what read_object gives back
+            return dequantize_fp8(*per_channel_fp8(tensor, dtype, spec.axis), spec.axis)
         scales, zps = per_channel_qparams(tensor, dtype, spec.axis)
         x = tensor.detach().float()
         return torch.quantize_per_channel(x, scales.to(x.device), zps.to(x.device), spec.axis, dtype)

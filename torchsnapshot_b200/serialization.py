@@ -65,6 +65,7 @@ class Serializer(Enum):
     BUFFER_PROTOCOL = "buffer_protocol"
     PER_TENSOR_QTENSOR = "per_tensor_qtensor"
     PER_CHANNEL_QTENSOR = "per_channel_qtensor"
+    PER_CHANNEL_FP8 = "per_channel_fp8"  # this package's scaled float8 format (per_channel_fp8_as_bytes)
 
 
 def _unsupported(what) -> ValueError:
@@ -190,3 +191,31 @@ def per_channel_qtensor_from_bytes(buf: bytes, dtype: torch.dtype, shape: List[i
     scales = tensor_from_memoryview(view[8 + body : 8 + body + 8 * channels], dtype=torch.float64, shape=[channels])
     zero_points = tensor_from_memoryview(view[8 + body + 8 * channels :], dtype=torch.int64, shape=[channels])
     return torch._make_per_channel_quantized_tensor(ints, scales, zero_points, axis)
+
+
+# ---- per-channel scaled float8 (this package's format; the reference has no reader for it) ------------------------
+#   [ axis: int64 ][ float8 bytes, C order ][ scales: float32 x shape[axis] ], little-endian
+def per_channel_fp8_as_bytes(q: torch.Tensor, scales: torch.Tensor, axis: int) -> bytes:
+    """The payload of a float8 tensor ``q`` with fp32 ``scales`` along ``axis`` (``prepare.per_channel_fp8`` gives both)."""
+    if q.dtype not in FLOAT8_DTYPES or scales.numel() != q.shape[axis]:
+        raise RuntimeError("per_channel_fp8_as_bytes() takes a float8 tensor and one scale per channel along axis.")
+    return _struct.pack("<q", axis) + bytes(tensor_as_memoryview(q.cpu())) + bytes(tensor_as_memoryview(scales.cpu().float()))
+
+
+def per_channel_fp8_from_bytes(buf: bytes, dtype: torch.dtype, shape: List[int]) -> torch.Tensor:
+    """The dequantised fp32 tensor of a per_channel_fp8 payload: ``q.float() * scale`` of its channel."""
+    from .prepare import dequantize_fp8
+
+    view = memoryview(buf)
+    axis = _struct.unpack("<q", view[:8])[0] if len(view) >= 8 else -1
+    if not 0 <= axis < len(shape):
+        raise RuntimeError(f"per_channel_fp8 header names axis {axis}, but the saved tensor has shape {list(shape)}")
+    body = 1
+    for s in shape:
+        body *= s
+    channels = shape[axis]
+    if dtype not in FLOAT8_DTYPES or len(view) != 8 + body + 4 * channels:
+        raise RuntimeError(f"The size of the buffer ({len(view)}) does not match the dtype/shape/axis.")
+    q = tensor_from_memoryview(view[8 : 8 + body], dtype=dtype, shape=shape)
+    scales = tensor_from_memoryview(view[8 + body :], dtype=torch.float32, shape=[channels])
+    return dequantize_fp8(q, scales, axis)
